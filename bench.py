@@ -13,6 +13,9 @@ queue per chunk: the two environment defaults set below, DESIGN.md section 4); S
 Seeds are independent: with N GPUs the 256 seeds are cut into blocks of ceil(256/N) per rank (SURVEY 8(e);
 "scaling": "strong"), no collective on the data path, one NCCL all_gather of the per-seed results at the end, inside
 the timed region (scptoolbox.jl_b200/sharded.py).  --weak keeps 256 seeds per GPU instead ("scaling": "weak").
+--dump-outputs DIR writes the whole-batch solution of the last timed step as DIR/<name>.npy (float64); the seeds are
+drawn from fixed random streams around a nominal guess computed on the CPU, so two builds run with the same arguments
+solve the same inputs and can be compared array for array.
 """
 from __future__ import annotations
 
@@ -55,6 +58,8 @@ def parse():
     ap.add_argument("--algo", default="ptr", choices=["ptr", "scvx", "gusto"],
                     help="ptr: the north-star workload (default); scvx: BASELINE configs[2], starship SCvx; "
                          "gusto: BASELINE configs[3], quadrotor obstacle avoidance with GuSTO")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the solution of the last timed step as DIR/<name>.npy (float64, at most 64 MiB)")
     a = ap.parse_args()
     dN, dNsub, dB = (60, 15, 1024) if a.algo == "gusto" else (100, 100, 256)
     a.N = a.N or dN; a.Nsub = a.Nsub or dNsub; a.batch = a.batch or dB
@@ -116,11 +121,30 @@ def effective_cores():
     return n
 
 
-def measured_peak():
-    try:
-        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+HBM_PEAK = (3350.0, "H100 SXM data sheet: 3.35 TB/s HBM3 at 700 W")
+
+
+DUMP_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(sol, out_dir):
+    """The arrays a caller of solve_sharded receives, as out_dir/<name>.npy in float64.  When they exceed DUMP_BYTES in
+    all, a fixed seeded sample of the seeds is written instead, with the sampled seed numbers in seed_index.npy."""
+    per_seed = {"xd": sol.xd, "ud": sol.ud, "p": sol.p, "cost": sol.cost, "deviation": sol.deviation,
+                "iterations": sol.iterations, "feas": sol.feas, "status": sol.raw_status}
+    per_seed = {k: np.asarray(v, dtype=np.float64) for k, v in per_seed.items()}
+    B = per_seed["cost"].shape[0]
+    td = np.asarray(sol.td, dtype=np.float64)
+    row = sum(a.nbytes for a in per_seed.values()) // B + 8
+    keep = (DUMP_BYTES - td.nbytes) // row
+    os.makedirs(out_dir, exist_ok=True)
+    if keep < B:
+        idx = np.sort(np.random.default_rng(0).choice(B, keep, replace=False))
+        per_seed = {k: v[idx] for k, v in per_seed.items()}
+        np.save(os.path.join(out_dir, "seed_index.npy"), idx.astype(np.float64))
+    for k, v in per_seed.items():
+        np.save(os.path.join(out_dir, f"{k}.npy"), v)
+    np.save(os.path.join(out_dir, "td.npy"), td)
 
 
 # PTR constants of the reference test (starship_flip/tests.jl:33-47)
@@ -330,14 +354,22 @@ def run_ours(args, rank, local_rank, world):
     else:
         pars = pkg.ptr.Parameters(N=N, Nsub=Nsub, disc_method=pkg.ptr.FOH, q_tr=np.inf, q_exit=np.inf,
                                   solver_opts={"verbose": 0, "maxit": 100}, **PTR)
-    base = traj.guess(N)                     # nominal guess (GPU SOCP batch); outside the timed region
+    if args.algo == "gusto":
+        base = traj.guess(N)                 # straight-line guess, computed on the host
+    else:
+        # nominal guess and seed scaling from the CPU restatement, as in the reference arm: the product's own generator
+        # solves an SOCP batch with the library under test, so two builds would start from different seeds and could not
+        # be compared output for output.  Outside the timed region.
+        from oracle import ptr as optr
+        pbo, base = oracle_base_guess(N)
+        mdl.hs = pbo.hs
+        sco = optr.Scaling(pbo, N)
     pbm = algo.create(pars, traj, h)
-    sc = pbm.scale
     if args.algo == "gusto":
         X, U, P = make_seeds_c4(base, Btot, 0, mdl.r0, mdl.rf)
         mdl.hs = 0.0
     else:
-        X, U, P = make_seeds(base, sc.Sx, sc.Su, Btot, 0, sc.cx, sc.cu)      # the whole batch, identical on every rank
+        X, U, P = make_seeds(base, sco.Sx, sco.Su, Btot, 0, sco.cx, sco.cu)      # the whole batch, identical on every rank
     lo, hi = pkg.sharded.shard_bounds(Btot, world, rank)
     Bloc = hi - lo
     info = pbm.cone.info()
@@ -385,6 +417,8 @@ def run_ours(args, rank, local_rank, world):
         dist.all_reduce(ln, op=dist.ReduceOp.SUM)
     dev_t, wall_t = float(t[0]), float(t[1])
     if rank == 0:
+        if args.dump_outputs:
+            dump_outputs(sol, args.dump_outputs)
         value = its / dev_t
         e2e = its / wall_t
         solved = sum(s_ == "SCP_SOLVED" for s_ in sol.status)
@@ -417,14 +451,7 @@ def run_ours(args, rank, local_rank, world):
             k_ms = 1e3 * phases["solve"] / max(lock, 1)
             ach = q_it * ipm / max(phases["solve"], 1e-12) / 1e9
             k_share = phases["solve"] / max(dev_t, 1e-12)
-        peak, peak_src = measured_peak()
-        traffic = None
-        for fn in ("r2_ipm_ncu_summary.json", "r1_ipm_ncu_summary.json"):
-            try:
-                traffic = json.load(open(os.path.join(ROOT, "profiles", fn)))["dram_bytes_per_launch"]
-                break
-            except Exception:
-                pass
+        peak, peak_src = HBM_PEAK
         # ---- roofline of K1 (k_discretize_foh): fp64-FMA bound; W from SURVEY 8(d), peak measured here ----
         ncalls = lock + args.steps                           # one discretize! per lock-step iteration + the initial guess
         w_seed = k1_flops_per_seed(N, Nsub, traj.nx, traj.nu, traj.np)
@@ -474,7 +501,7 @@ def run_ours(args, rank, local_rank, world):
                 "ms_per_socp_solve": k_ms,
                 "phase_seconds_per_step": {k: v / args.steps for k, v in phases.items()},
                 "roofline": {"bound": "hbm", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                             "traffic": traffic, "peak_source": peak_src, "kernel": "k_ipm_solve",
+                             "traffic": None, "peak_source": peak_src, "kernel": "k_ipm_solve",
                              "kernel_ms": k_ms, "algorithmic_bytes_per_ipm_iteration_per_seed": q_it,
                              "ipm_iterations_per_launch": ipm / max(lock, 1), "ldl_solves_per_ipm_iteration": nsolve,
                              "kernel_share_of_step": k_share,

@@ -1,4 +1,4 @@
-/* scpb.h -- C ABI of libscpb (B200-native SCP inner loop).
+/* scpb.h -- C ABI of libscpb (CUDA SCP inner loop for the H100, sm_90a).
  *
  * Drop-in boundary for the hot path of UW-ACL/SCPToolbox.jl (file:line relative to the
  * reference tree):

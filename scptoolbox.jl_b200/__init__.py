@@ -1,4 +1,4 @@
-"""scptoolbox.jl_b200 -- B200-native SCP inner loop (discretize! + subproblem solve) behind a C ABI.
+"""scptoolbox.jl_b200 -- CUDA SCP inner loop for the H100 (discretize! + subproblem solve) behind a C ABI.
 
 The directory name carries a dot, so the package is imported under the alias
 `scptoolbox_jl_b200` (see __graft_entry__.load_package()).

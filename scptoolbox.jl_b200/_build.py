@@ -1,4 +1,4 @@
-"""Build libscpb.so (sm_100a) in-tree with nvcc.  Called by __graft_entry__.build()."""
+"""Build libscpb.so (sm_90a, H100) in-tree with nvcc.  Called by __graft_entry__.build()."""
 from __future__ import annotations
 
 import glob
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SO = os.path.join(HERE, "libscpb.so")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
 

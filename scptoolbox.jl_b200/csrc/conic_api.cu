@@ -58,7 +58,7 @@ __global__ void k_from_grouped(const double *src, double *dst, int E, int B, int
     dst[(size_t)sd * E + e] = src[((size_t)(sd / G) * E + e) * G + (sd % G)];
 }
 
-int scpb_internal_pick_group(int B, int want)
+int scpb_internal_pick_group(int B, int want, int sms)
 {
     if (want > 0) {
         int g = 1;
@@ -66,7 +66,7 @@ int scpb_internal_pick_group(int B, int want)
         return g;
     }
     int g = 1;
-    while ((B + g - 1) / g > 148 && g < IPM_MAXG) g <<= 1;   // one persistent CTA per SM
+    while ((B + g - 1) / g > sms && g < IPM_MAXG) g <<= 1;   // one persistent CTA per SM
     return g;
 }
 
@@ -110,6 +110,7 @@ static int cone_reserve(scpb_cone_s *c, int B, int G)
     D.soceta = al(S.nsoc + 1);
     D.dx = al(n); D.dy = al(p); D.dz = al(m); D.ds = al(m); D.dsa = al(m); D.dza = al(m); D.tm = al(m); D.gm = al(m);
     D.r1 = al(n); D.r2 = al(p); D.e1 = al(nm); D.e2 = al(p); D.rhs = al(nk);
+    D.part = al(S.npart); D.pcnt = al(S.npart);
     D.Y = al(std::max<size_t>((size_t)S.nnzL + nk, (size_t)S.sn_panel_size)); D.Ls = al(S.nnzL + 1); D.Lrow = al(S.nnzL + 1); D.invD = al(nk);
     bool ok = true;
     for (double *q : c->bufs) ok = ok && q != nullptr;
@@ -117,7 +118,10 @@ static int cone_reserve(scpb_cone_s *c, int B, int G)
          cudaMalloc((void **)&c->d_iters, sizeof(int) * Bpad) == cudaSuccess &&
          cudaMalloc((void **)&c->d_scal, sizeof(double) * 5 * Bpad) == cudaSuccess &&
          cudaMalloc((void **)&c->d_warm, sizeof(int) * Bpad) == cudaSuccess &&
-         cudaMemset(c->d_warm, 0, sizeof(int) * Bpad) == cudaSuccess;
+         cudaMemsetAsync(c->d_warm, 0, sizeof(int) * Bpad, h->stream) == cudaSuccess &&
+         // split-target counters start at zero; on the handle's stream, which the solver launches (and the chunk
+         // streams of ptr.cu) are ordered after
+         cudaMemsetAsync(D.pcnt, 0, sizeof(double) * ((size_t)S.npart + 1) * Bpad, h->stream) == cudaSuccess;
     if (!ok) {
         cudaGetLastError();
         for (double *q : c->bufs) if (q) cudaFree(q);
@@ -154,15 +158,14 @@ int scpb_internal_cone_run(scpb_cone_s *c, const IpmOpts &o, const int *skip, cu
     if (ng <= 0) return SCPB_OK;
     c->D.g0 = ngc > 0 ? g0 : 0;
     // dynamic shared memory: level pointers (+ the substitution vector when nk*G doubles fit next to the
-    // ~20 KB of static shared memory; B200 allows 227 KB per CTA)
+    // ~20 KB of static shared memory; H100 allows 227 KB per CTA)
     size_t smem = sizeof(int) * ((9 * (size_t)(c->S.nlevels + 1) + 3) & ~(size_t)3);
     const size_t vbytes = sizeof(double) * (size_t)c->S.nk * c->D.G;
     c->D.vsmem = (smem + vbytes <= 200 * 1024 && !getenv("SCPB_NO_VSMEM")) ? 1 : 0;   // env: force the global-memory sweep (tests)
     if (c->D.vsmem) smem += vbytes;
     // supernodal factorisation / substitutions (csrc/conic_sn.cuh), SCPB_SUPERNODAL=1: every panel must fit a lane
     // group and the substitution vector must live in shared memory.  Correct on the device (tests/test_conic_gpu.py)
-    // but measured slower than the scalar level-scheduled programs on the bench KKT (profiles/r2_experiments.md), so
-    // the scalar programs stay the default.
+    // but slower than the scalar level-scheduled programs on the bench KKT, so the scalar programs stay the default.
     {
         const char *e = getenv("SCPB_SUPERNODAL");
         c->D.sn = (c->sn_ok && c->D.vsmem && e && e[0] == '1') ? 1 : 0;
@@ -229,9 +232,9 @@ IpmOpts scpb_internal_make_opts(const scpb_cone_opts *o)
 }
 
 // PTR loop: early interior-point iterations only need a direction, so refinement stops two digits below the requested
-// feasibility (inside [1e-13, 1e-11]) while gap/deg > 1e-6 and at 1e-13 below that -- measured on the bench: 2.06 instead of
-// 2.19 LDL' solves per iteration, the same iteration counts, -10 % solve time (profiles/r2_experiments.md section 4).  With
-// 1e-11 all the way one of the N = 31 starship test programs stalled at a relative gap of 1e-6, hence the switch.
+// feasibility (inside [1e-13, 1e-11]) while gap/deg > 1e-6 and at 1e-13 below that -- on the bench seeds 2.06 instead of
+// 2.19 LDL' solves per interior-point iteration with the same iteration counts.  With 1e-11 all the way one of the
+// N = 31 starship test programs stalled at a relative gap of 1e-6, hence the switch.
 void scpb_internal_relax_refinement(IpmOpts &r)
 {
     if (getenv("SCPB_REFTOL")) return;
@@ -302,6 +305,8 @@ int32_t scpb_cone_setup(scpb_handle h, int32_t n, int32_t p, int32_t m, const in
     P.fwp_lvl = upload_ints(c, S.fwp_lvl); P.bwp_lvl = upload_ints(c, S.bwp_lvl);
     P.fwp_R = upload_ints(c, S.fwp_R); P.bwp_R = upload_ints(c, S.bwp_R);
     P.Lr_pc = (const int2 *)upload_ints(c, S.Lr_pc); P.ft_op = (const int2 *)upload_ints(c, S.ft_op);
+    P.fc_item = (const int4 *)upload_ints(c, S.fc_item); P.fwc_item = (const int4 *)upload_ints(c, S.fwc_item);
+    P.bwc_item = (const int4 *)upload_ints(c, S.bwc_item);
     // hybrid program: SCPB_HYBRID=<cut> (supernodal level at which the in-place panels take over; 0 = off)
     {
         const char *e = getenv("SCPB_HYBRID");
@@ -316,11 +321,15 @@ int32_t scpb_cone_setup(scpb_handle h, int32_t n, int32_t p, int32_t m, const in
             H.fwp_item = (const int4 *)upload_ints(c, S.hy_fwp_item); H.bwp_item = (const int4 *)upload_ints(c, S.hy_bwp_item);
             H.fwp_lvl = upload_ints(c, S.hy_fwp_lvl); H.bwp_lvl = upload_ints(c, S.hy_bwp_lvl);
             H.fwp_R = upload_ints(c, S.hy_fwp_R); H.bwp_R = upload_ints(c, S.hy_bwp_R);
+            H.fc_item = (const int4 *)upload_ints(c, S.hy_fc_item); H.fwc_item = (const int4 *)upload_ints(c, S.hy_fwc_item);
+            H.bwc_item = (const int4 *)upload_ints(c, S.hy_bwc_item);
             H.hy.desc = (const int4 *)upload_ints(c, S.hy_desc); H.hy.tl_ptr = upload_ints(c, S.hy_tl_ptr);
             H.hy.upd_dst = upload_ints(c, S.hy_upd_dst); H.hy.rows = P.sn.rows; H.hy.ntl = S.hy_ntl;
             c->hy_ok = true;
         }
     }
+    P.npart = S.npart;   // the hybrid program's slots are counted in S.npart too
+    c->P_hy.npart = S.npart;
     for (void *d : c->dev_ints)
         if (!d) {
             scpb_cone_free(c);
@@ -375,7 +384,7 @@ int32_t scpb_debug_kkt_solve_dev(scpb_cone c, int32_t B, const double *Avals, co
     if (!c || B <= 0 || !wm || !rhs || !sol) return SCPB_ERR_ARG;
     scpb_handle_s *h = c->h;
     SCPB_CUDA(h, cudaSetDevice(h->device));
-    const int G = scpb_internal_pick_group(B, 0);
+    const int G = scpb_internal_pick_group(B, 0, h->sms);
     int rc = cone_reserve(c, B, G);
     if (rc) return rc;
     const ConeSymbolic &S = c->S;
@@ -451,7 +460,7 @@ int32_t scpb_cone_solve(scpb_cone c, int32_t B, const double *Avals, const doubl
     scpb_handle_s *h = c->h;
     if (B <= 0 || !cvec || (c->S.p > 0 && !bvec) || (c->S.m > 0 && !hvec)) return set_err(h, SCPB_ERR_ARG, "cone_solve: bad arguments");
     SCPB_CUDA(h, cudaSetDevice(h->device));
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0);
+    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
     c->lanes = opts ? opts->lanes : 0;
     int rc = cone_reserve(c, B, G);
     if (rc) return rc;

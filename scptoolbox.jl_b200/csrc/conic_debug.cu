@@ -5,6 +5,37 @@
 #include "../../include/scpb.h"
 #include "conic_symbolic.h"
 
+// An item's partial sum, applied the way k_ipm_solve applies it: straight to the target, or, for an item of a split
+// target (.w = 1 + slot, conic_symbolic.h: number_pieces), into its slot, the last item of the target subtracting the
+// slots in slot order.  add() fails when the slot does not belong to the item's target; level_done() fails when a
+// target of the level did not receive all the items its slot range promises.
+struct SplitSums {
+    std::vector<double> part;
+    std::vector<int> cnt;
+    explicit SplitSums(int npart) : part((size_t)npart + 1, 0.0), cnt((size_t)npart + 1, 0) {}
+    bool add(const int *it, const std::vector<int> &info, double p, double *y)
+    {
+        if (!it[3]) { y[it[0]] -= p; return true; }
+        const int sl = it[3] - 1;
+        if (sl < 0 || 4 * (size_t)sl + 3 >= info.size()) return false;
+        const int *e = &info[4 * (size_t)sl];
+        if (e[0] != it[0] || sl < e[1] || sl >= e[2]) return false;
+        part[sl] = p;
+        if (++cnt[e[1]] == e[2] - e[1]) {
+            double acc = y[e[0]];
+            for (int k = e[1]; k < e[2]; k++) acc -= part[k];
+            y[e[0]] = acc;
+            cnt[e[1]] = 0;
+        }
+        return true;
+    }
+    bool level_done() const
+    {
+        for (int c : cnt) if (c) return false;
+        return true;
+    }
+};
+
 extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const int32_t *A_rp, const int32_t *A_ci,
                                         const int32_t *G_rp, const int32_t *G_ci, int32_t l, int32_t nsoc,
                                         const int32_t *soc_dims, const int32_t *perm, const double *Av,
@@ -23,6 +54,8 @@ extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const i
         for (int k = S.as_ptr[t]; k < S.as_ptr[t + 1]; k++) acc += Gv[S.as_a[k]] * Gv[S.as_b[k]] * wm[S.as_c[k]];
         Y[t] = acc;
     }
+    SplitSums split(S.npart);
+    int64_t nsplit = 0;
     for (int lv = 0; lv < S.nlevels; lv++) {  // kkt_factor: balanced program (phase A items, then phase B items)
         const int R = S.fa_R[lv];
         for (int w = S.fa_lvl[lv]; w < S.fa_lvl[lv + 1]; w++) {
@@ -30,8 +63,10 @@ extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const i
             if (it[2] - it[1] > R * CONIC_FACTOR_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Y[S.ft_op[2 * (size_t)k]] * Ls[S.Lr_pos[S.ft_op[2 * (size_t)k + 1]]];
-            Y[it[0]] -= part;
+            if (!split.add(it, S.fc_item, part, Y.data())) return SCPB_ERR_ARG;
+            nsplit += it[3] != 0;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.fb_lvl[lv]; w < S.fb_lvl[lv + 1]; w++) {   // every item regularises its own copy of the pivot
             const int *it = &S.fb_item[4 * (size_t)w];
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;
@@ -53,8 +88,10 @@ extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const i
             if (it[2] - it[1] > R * CONIC_SOLVE_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Lrow[k] * v[S.Lr_col[k]];
-            v[it[0]] -= part;
+            if (!split.add(it, S.fwc_item, part, v.data())) return SCPB_ERR_ARG;
+            nsplit += it[3] != 0;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int i = 0; i < nk; i++) v[i] *= invD[i];
     for (int lv = S.nlevels - 1; lv >= 0; lv--) {
@@ -64,11 +101,13 @@ extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const i
             if (it[2] - it[1] > R * CONIC_SOLVE_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Ls[k] * v[S.L_ri[k]];
-            v[it[0]] -= part;
+            if (!split.add(it, S.bwc_item, part, v.data())) return SCPB_ERR_ARG;
+            nsplit += it[3] != 0;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int i = 0; i < nk; i++) sol[i] = v[S.iperm[i]];
-    if (info) { info[0] = S.nnzL; info[1] = S.nlevels; info[2] = S.factor_ops; info[3] = (int64_t)S.as_a.size(); }
+    if (info) { info[0] = S.nnzL; info[1] = S.nlevels; info[2] = S.factor_ops; info[3] = (int64_t)S.as_a.size(); info[4] = nsplit; }
     return SCPB_OK;
 }
 
@@ -175,6 +214,7 @@ extern "C" int32_t scpb_debug_kkt_solve_hy(int32_t n, int32_t p, int32_t m, cons
         for (int k = S.as_ptr[t]; k < S.as_ptr[t + 1]; k++) acc += Gv[S.as_a[k]] * Gv[S.as_b[k]] * wm[S.as_c[k]];
         Y[t] = acc;
     }
+    SplitSums split(S.npart);
     for (int lv = 0; lv < nl; lv++) {  // low columns + bridge level: the scalar balanced programs
         const int R = S.hy_fa_R[lv];
         for (int w = S.hy_fa_lvl[lv]; w < S.hy_fa_lvl[lv + 1]; w++) {
@@ -182,8 +222,9 @@ extern "C" int32_t scpb_debug_kkt_solve_hy(int32_t n, int32_t p, int32_t m, cons
             if (it[2] - it[1] > R * CONIC_FACTOR_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Y[S.hy_ft_op[2 * (size_t)k]] * Ls[S.Lr_pos[S.hy_ft_op[2 * (size_t)k + 1]]];
-            Y[it[0]] -= part;
+            if (!split.add(it, S.hy_fc_item, part, Y.data())) return SCPB_ERR_ARG;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.hy_fb_lvl[lv]; w < S.hy_fb_lvl[lv + 1]; w++) {
             const int *it = &S.hy_fb_item[4 * (size_t)w];
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;
@@ -234,8 +275,9 @@ extern "C" int32_t scpb_debug_kkt_solve_hy(int32_t n, int32_t p, int32_t m, cons
             if (it[2] - it[1] > R * CONIC_SOLVE_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Lrow[k] * v[S.Lr_col[k]];
-            v[it[0]] -= part;
+            if (!split.add(it, S.hy_fwc_item, part, v.data())) return SCPB_ERR_ARG;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int tl = 0; tl < S.hy_ntl; tl++)   // forward through the top panels (column oriented)
         for (int q = S.hy_tl_ptr[tl]; q < S.hy_tl_ptr[tl + 1]; q++) {
@@ -266,8 +308,9 @@ extern "C" int32_t scpb_debug_kkt_solve_hy(int32_t n, int32_t p, int32_t m, cons
             if (it[2] - it[1] > R * CONIC_SOLVE_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Ls[k] * v[S.L_ri[k]];
-            v[it[0]] -= part;
+            if (!split.add(it, S.hy_bwc_item, part, v.data())) return SCPB_ERR_ARG;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int i = 0; i < nk; i++) sol[i] = v[S.iperm[i]];
     if (info) {
@@ -333,13 +376,15 @@ extern "C" int32_t scpb_debug_kkt_factor(void *h, const double *Av, const double
     }
     int nbad = 0, nreg = 0;
     double lmax = 0.0, dmin = 1e300;
+    SplitSums split(S.npart);
     for (int lv = 0; lv < S.nlevels; lv++) {
         for (int w = S.fa_lvl[lv]; w < S.fa_lvl[lv + 1]; w++) {
             const int *it = &S.fa_item[4 * (size_t)w];
             double part = 0.0;
             for (int q = it[1]; q < it[2]; q++) part += Y[S.ft_op[2 * (size_t)q]] * Ls[S.Lr_pos[S.ft_op[2 * (size_t)q + 1]]];
-            Y[it[0]] -= part;
+            if (!split.add(it, S.fc_item, part, Y.data())) return SCPB_ERR_ARG;
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.fb_lvl[lv]; w < S.fb_lvl[lv + 1]; w++) {
             const int *it = &S.fb_item[4 * (size_t)w];
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;

@@ -6,7 +6,7 @@
 // KKT system, iterative refinement) -- ECOS is an unvendored dependency of the reference, so this
 // is written from the published algorithm (Domahidi et al. 2013; CVXOPT conelp), not from its code.
 //
-// B200 execution model: seeds are independent, so ALL synchronisation is kept inside a CTA.
+// Execution model: seeds are independent, so ALL synchronisation is kept inside a CTA.
 // One persistent CTA owns a group of G seeds and runs the complete interior-point solve for them:
 // residual SpMVs, cone scaling, KKT assembly, numeric LDL', triangular solves, line search.
 // Every sparse operation is a "gather program" generated on the host from the shared pattern
@@ -38,6 +38,8 @@ struct IpmProgram {  // device copies of ConeSymbolic index arrays
     const int *fa_lvl, *fa_R, *fb_lvl;
     const int *fwp_lvl, *bwp_lvl, *fwp_R, *bwp_R;
     const int2 *Lr_pc, *ft_op;
+    const int4 *fc_item, *fwc_item, *bwc_item;   // per partial-sum slot: {target, first slot, end slot, 0} (conic_symbolic.h)
+    int npart;                                   // partial-sum slots per seed
 };
 
 struct IpmOpts {
@@ -72,6 +74,8 @@ struct IpmData {  // group-blocked device arrays, all for B seeds
     // work
     double *rx, *ry, *rz, *lam, *wm, *socw, *soceta;
     double *dx, *dy, *dz, *ds, *dsa, *dza, *tm, *gm, *r1, *r2, *e1, *e2, *rhs, *Y, *Ls, *Lrow, *invD;
+    double *part;   // partial sums of split targets (IpmProgram.npart slots per seed)
+    double *pcnt;   // storage of the split targets' finished-item counters (unsigned, zero between uses)
     int vsmem;   // 1: the substitution vector of kkt_ldl_solve lives in shared memory (nk*G doubles fit)
     // per-seed outputs
     double *pobj, *dobj, *res;   // res: [3][B] pres, dres, gap
@@ -116,6 +120,8 @@ struct Ctx {
     double rho_min, bad_abs;
     double *vs;                         // shared-memory substitution vector (nullptr: use global memory)
     double *Lrow;                       // row-ordered copy of the scaled factor (forward substitution)
+    double *part;                       // partial sums of the split targets of a level
+    unsigned *pcnt;                     // ... and their finished-item counters
     double reftol;                      // iterative refinement stops once |residual|_inf <= reftol*(1+|rhs|_inf) ...
     const double *s_mu;                 // ... reftol while the seed's complementarity gap/deg is above mu_tight, 1e-13 below it
     double mu_tight;                    //     (shared: per-seed mu of the current iterate)
@@ -174,8 +180,8 @@ __device__ __forceinline__ double lanes_sum(const Ctx &c, double a)
 }
 
 // y = alpha * (M x) [+ y0]  row-wise CSR; M values Mv group-blocked
-// (chunked variants with four entries in flight were measured and are slower: inside the solver body the 64-register
-// budget of a 1024-thread CTA spills them, profiles/r2_experiments.md)
+// (chunked variants with four entries in flight are slower: inside the solver body the 64-register budget of a
+// 1024-thread CTA spills them)
 __device__ __forceinline__ double row_dot(const int *rp, const int *ci, const double *Mv, const double *x, int r,
                                           int G, int sg)
 {
@@ -248,16 +254,35 @@ __device__ __forceinline__ void kkt_assemble(const IpmProgram &P, const Ctx &c, 
 // ---- numeric LDL' : balanced, level-scheduled gather program (conic_symbolic.h, "balanced factorisation program") ----
 // Phase A of a level: an item subtracts at most R*IPM_FPF products Y[a]*Ls[b] from one target; a lane owns at most
 // IPM_FPF of them, so all its op indices and then all its gathers are in flight together.  Targets whose op list was
-// split receive their partial sums through global atomics (hence every read of Y goes to L2, ld.cg).  Phase B finishes
+// split store their partial sums in slots that the last of them subtracts in slot order (ipm_split_done; every read of Y
+// goes to L2, ld.cg).  Phase B finishes
 // the level's columns: each item regularises its own copy of the pivot, the diagonal item stores 1/d, the others
 // scale their entry and store it twice (column order for the backward sweep, row order for the forward sweep).
 // The program data of the next phase (item descriptors, op indices) is requested one phase early.
 // Separate (noinline) function with by-value arguments: see solve_sweep.
 #define IPM_FPF CONIC_FACTOR_PF
+// An item of a split target stores its partial sum in its slot and counts itself in; the last item of the target to
+// finish subtracts all slots from the target in slot order (and resets the counter), so the sum does not depend on the
+// order in which the items ran.  Returns true in the thread that has to do that.
+__device__ __forceinline__ bool ipm_split_done(double *part, unsigned *cnt, int4 e, int sl, double v, int G, int sg)
+{
+    part[(size_t)sl * G + sg] = v;
+    __threadfence_block();
+    const bool last = atomicAdd(&cnt[(size_t)e.y * G + sg], 1u) == (unsigned)(e.z - e.y - 1);
+    if (last) { __threadfence_block(); cnt[(size_t)e.y * G + sg] = 0u; }
+    return last;
+}
+__device__ __forceinline__ double ipm_split_sum(const double *part, int4 e, double acc, int G, int sg)
+{
+    for (int k = e.y; k < e.z; k++) acc -= __ldcg(&part[(size_t)k * G + sg]);
+    return acc;
+}
 struct FactorArgs {
     const int4 *fa_item, *fb_item;
     const int2 *ft_op;
-    double *Y, *Ls, *Lrow, *invD;   // group-blocked, already offset to this CTA's group
+    const int4 *fc_item;            // partial-sum slots of the split targets
+    double *Y, *Ls, *Lrow, *invD, *part;   // group-blocked, already offset to this CTA's group
+    unsigned *pcnt;
     int o_fal, o_faR, o_fbl;        // offsets (ints) into the dynamic shared memory window
     int nl, nnzLd, G, sg, slot, nslots;
     long long *lprof;
@@ -278,7 +303,7 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
     const int G = a.G, sg = a.sg, slot = a.slot, nslots = a.nslots;
     // three-stage software pipeline over the passes of phase A: the item descriptor of pass p+2 and the op indices of
     // pass p+1 are requested while the gathers of pass p are in flight, so a pass costs one memory latency
-    int t_tgt;                 // current pass: target | split << 30, or -1
+    int t_tgt;                 // current pass: target, or partial-sum slot | 1 << 30 for a split target, or -1
     int2 t_op[IPM_FPF];        // current pass: op indices of this lane (x < 0: none)
     int i_tgt, i_k0, i_k1;     // next pass: item descriptor (k0 already offset to this lane)
 #define IPM_FA_ITEM(LV, OFF)                                                              \
@@ -288,7 +313,8 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
         i_tgt = -1; i_k0 = 0; i_k1 = 0;                                                   \
         if ((OFF) < fal[(LV) + 1] - fal[LV] && w_ < fal[(LV) + 1]) {                      \
             const int4 it_ = a.fa_item[w_];                                               \
-            i_tgt = it_.x | (it_.w << 30); i_k0 = it_.y + (slot & (R_ - 1)); i_k1 = it_.z; \
+            i_tgt = it_.w ? ((it_.w - 1) | (1 << 30)) : it_.x;                              \
+            i_k0 = it_.y + (slot & (R_ - 1)); i_k1 = it_.z;                               \
         }                                                                                 \
     }
 #define IPM_FA_OPS(TGT, OP, R_)                                                           \
@@ -326,8 +352,14 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
             for (int j = 0; j < IPM_FPF; j++) part_ = fma(ya_[j], la_[j], part_);
             for (int o_ = G; o_ < G * R; o_ <<= 1) part_ += __shfl_xor_sync(0xffffffffu, part_, o_);
             if (t_tgt >= 0 && (slot & (R - 1)) == 0) {
-                double *p_ = &a.Y[(size_t)(t_tgt & 0x3fffffff) * G + sg];
-                if (t_tgt >> 30) atomicAdd(p_, -part_); else *p_ = __ldcg(p_) - part_;
+                if (t_tgt >> 30) {
+                    const int sl_ = t_tgt & 0x3fffffff;
+                    const int4 e_ = a.fc_item[sl_];
+                    if (ipm_split_done(a.part, a.pcnt, e_, sl_, part_, G, sg)) {
+                        double *p_ = &a.Y[(size_t)e_.x * G + sg];
+                        *p_ = ipm_split_sum(a.part, e_, __ldcg(p_), G, sg);
+                    }
+                } else { double *p_ = &a.Y[(size_t)t_tgt * G + sg]; *p_ = __ldcg(p_) - part_; }
             }
             t_tgt = n_tgt;
 #pragma unroll
@@ -547,8 +579,8 @@ __device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *
 {
     if constexpr (SN == 1) { kkt_factor_sn(c.s_sn, c.tid); return; }
     FactorArgs a;
-    a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op;
-    a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD;
+    a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fc_item = P.fc_item;
+    a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.part; a.pcnt = c.pcnt;
     a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
     a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = c.G; a.sg = c.sg; a.slot = c.slot; a.nslots = c.nslots;
     a.lprof = c.lprof;
@@ -561,7 +593,7 @@ __device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *
 // R*IPM_PF entries (conic_symbolic.h, "balanced substitution programs"), so a lane never owns more than IPM_PF
 // entries of an item: right after a level's items are consumed the lane issues ALL global loads of the next level
 // (indices + values, through an item descriptor fetched one level earlier) and only then waits at the barrier.
-// Items of a split row combine their partial sums with shared-memory atomics.
+// Items of a split row store their partial sums in slots that the last of them subtracts in slot order.
 // The sweep is a separate (noinline) function with by-value arguments and shared-window pointers: its register
 // allocation is independent of the 60+ live pointers of the solver body, so the prefetch registers are not spilled
 // (a spilled prefetch is a synchronous load).
@@ -570,15 +602,13 @@ struct SweepArgs {
     const int4 *items;      // balanced items {node, start, end, split}
     const int *idxarr;      // entry -> vector index (column of the row entry / row of the column entry)
     const double *vals;     // group-blocked L values in the same entry order
+    const int4 *cmb;        // partial-sum slots of the split rows / columns
+    double *part;           // group-blocked partial-sum slots and their counters
+    unsigned *pcnt;
     int o_lvl, o_R, o_vs;   // offsets (ints) into the dynamic shared memory window
     int nl, lv0, G, sg, slot, nslots;
     long long *lprof;       // per-level cycle counters (CTA 0, thread 0) or nullptr
 };
-
-__device__ __forceinline__ double smem_atomic_add(double *addr, double v)
-{
-    return atomicAdd(addr, v);   // addr is derived from ipm_smem: the compiler emits the shared-space form
-}
 
 template <int DIR>
 __device__ __noinline__ void solve_sweep(const SweepArgs a)
@@ -589,9 +619,9 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
     const int G = a.G, sg = a.sg, slot = a.slot;
     const int nsteps = DIR > 0 ? a.nl - a.lv0 : a.lv0 + 1;
     if (nsteps <= 0) return;
-    // item descriptor of this lane for the level after next; (node | split << 30), first entry, end
+    // item descriptor of this lane for the level after next; node (or partial-sum slot | 1 << 30), first entry, end
     int i_node, i_k0, i_k1, i_R;
-    int q_node;                    // current item: node | split << 30, or -1
+    int q_node;                    // current item: node, or slot | 1 << 30 for a split row, or -1
     int q_idx[IPM_PF];
     double q_val[IPM_PF];
 #define IPM_ITEM_LOAD(LV, OFF)                                                            \
@@ -601,7 +631,8 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
         i_node = -1; i_R = R_; i_k0 = 0; i_k1 = 0;                                        \
         if (w_ < lvl[(LV) + 1]) {                                                         \
             const int4 it_ = a.items[w_];                                                 \
-            i_node = it_.x | (it_.w << 30); i_k0 = it_.y + (slot & (R_ - 1)); i_k1 = it_.z; \
+            i_node = it_.w ? ((it_.w - 1) | (1 << 30)) : it_.x;                             \
+            i_k0 = it_.y + (slot & (R_ - 1)); i_k1 = it_.z;                               \
         }                                                                                 \
     }
 #define IPM_VALS_LOAD()                                                                   \
@@ -620,8 +651,12 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
         _Pragma("unroll") for (int j = 0; j < IPM_PF; j++) part_ = fma(q_val[j], vs[q_idx[j] * G + sg], part_); \
         for (int o_ = G; o_ < G * (R); o_ <<= 1) part_ += __shfl_xor_sync(0xffffffffu, part_, o_); \
         if (q_node >= 0 && (slot & ((R) - 1)) == 0) {                                     \
-            double *t_ = &vs[(q_node & 0x3fffffff) * G + sg];                             \
-            if (q_node >> 30) smem_atomic_add(t_, -part_); else *t_ -= part_;             \
+            if (q_node >> 30) {                                                           \
+                const int sl_ = q_node & 0x3fffffff;                                      \
+                const int4 e_ = a.cmb[sl_];                                               \
+                if (ipm_split_done(a.part, a.pcnt, e_, sl_, part_, G, sg))                \
+                    vs[e_.x * G + sg] = ipm_split_sum(a.part, e_, vs[e_.x * G + sg], G, sg); \
+            } else vs[q_node * G + sg] -= part_;                                          \
         }                                                                                 \
     }
     IPM_ITEM_LOAD(a.lv0, 0)
@@ -661,9 +696,10 @@ __device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c, 
     const long long t0_ = clock64();
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
     SweepArgs a;
-    a.nl = P.nlevels; a.G = G; a.sg = sg; a.slot = c.slot; a.nslots = c.nslots; a.o_vs = c.o_vs;
+    a.nl = P.nlevels; a.G = G; a.sg = sg; a.slot = c.slot; a.nslots = c.nslots; a.o_vs = c.o_vs; a.part = c.part; a.pcnt = c.pcnt;
     // forward: level 0 rows are empty (leaves have no dependencies); the barrier inside the sweep publishes vs
     a.items = P.fwp_item; a.idxarr = P.Lr_col; a.vals = c.Lrow; a.o_lvl = c.o_fwl; a.o_R = c.o_fwR; a.lv0 = 1;
+    a.cmb = P.fwc_item;
     a.lprof = c.lprof ? c.lprof + P.nlevels : nullptr;
     solve_sweep<1>(a);
     if (P.nlevels <= 1) __syncthreads();
@@ -673,6 +709,7 @@ __device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c, 
     if constexpr (SN == 2) { __syncthreads(); kkt_sweep_top<-1>(c.s_hy, c.tid); }
     // backward: the top level holds roots only (empty columns)
     a.items = P.bwp_item; a.idxarr = P.L_ri; a.vals = Ls; a.o_lvl = c.o_bwl; a.o_R = c.o_bwR; a.lv0 = P.nlevels - 2;
+    a.cmb = P.bwc_item;
     a.lprof = c.lprof ? c.lprof + 2 * P.nlevels : nullptr;
     solve_sweep<-1>(a);
     if (P.nlevels <= 1) __syncthreads();
@@ -1131,6 +1168,8 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         s_snargs = a;
     }
     c.Lrow = GP(D.Lrow, P.nnzL + 1);
+    c.part = GP(D.part, P.npart + 1);
+    c.pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
 #undef GP
 
     long long pt[8] = {0, 0, 0, 0, 0, 0, 0, 0};

@@ -76,16 +76,20 @@ struct ConeSymbolic {
     std::vector<int> lvl_maxlen;         // [3][nlevels]: longest L row / L column / factor op list of each level
     // balanced substitution programs: every item covers at most R*SOLVE_PF entries of one row (forward) / column
     // (backward), R = lanes per item of that level; rows longer than that are split into several items whose partial
-    // sums are combined with atomics (flag in .w).  All loads of an item fit the per-lane register prefetch.
-    std::vector<int> fwp_item, bwp_item; // int4 {node, start, end, split}
+    // sums are combined in a fixed order by the last of them to finish (.w = 1 + partial-sum slot, see number_pieces).
+    // All loads of an item fit the per-lane register prefetch.
+    std::vector<int> fwp_item, bwp_item; // int4 {node, start, end, 0 | 1 + slot}
     std::vector<int> fwp_lvl, bwp_lvl;   // nlevels+1 -> index into the item lists
     std::vector<int> fwp_R, bwp_R;       // lanes per item of each level
     // balanced factorisation program, same idea: phase A items cover at most R*CONIC_FACTOR_PF ops of one target
-    // (Y[target] -= sum Y[a]*Ls[b]; split targets use atomics; targets without ops have no item), phase B items
+    // (Y[target] -= sum Y[a]*Ls[b]; split targets are combined like the substitution's; targets without ops have no item), phase B items
     // finish a column: {Y position, column, row-order position, flags}; flags bit0 = expected pivot sign is +,
     // bit1 = the item is the diagonal itself (regularise, write 1/d), otherwise scale the entry by 1/d.
     std::vector<int> fa_item, fa_lvl, fa_R;
     std::vector<int> fb_item, fb_lvl;
+    // partial-sum slots of the split targets: int4 per slot {target, first slot, end slot of the target, 0} (number_pieces)
+    std::vector<int> fc_item, fwc_item, bwc_item;
+    int npart = 0;                    // partial-sum slots per seed: the most any of the programs (hybrid included) uses
     // ---- supernodal program (executed by the kernels of conic_sn.cuh; CPU interpreter scpb_debug_kkt_solve_sn,
     // tests/test_conic_symbolic.py) ----
     // Maximal supernodes: consecutive columns a..b with parent(j) = j+1 and struct(L[:,j]) = {j+1} + struct(L[:,j+1]);
@@ -112,6 +116,7 @@ struct ConeSymbolic {
     int hy_cut = 0, hy_nlevels = 0, hy_ntl = 0;
     std::vector<int> hy_fa_item, hy_fa_lvl, hy_fa_R, hy_fb_item, hy_fb_lvl, hy_ft_op;
     std::vector<int> hy_fwp_item, hy_fwp_lvl, hy_fwp_R, hy_bwp_item, hy_bwp_lvl, hy_bwp_R;
+    std::vector<int> hy_fc_item, hy_fwc_item, hy_bwc_item;
     std::vector<int> hy_tl_ptr;     // hy_ntl + 1 -> index into the descriptor list
     std::vector<int> hy_desc;       // 8 ints per top supernode in top-level order: {first column, width, rows, L_cp[first]},
                                     // {offset into sn_rows, offset into hy_upd_dst, pivot signs (bit c: column c expects +), 0}
@@ -125,6 +130,32 @@ struct ConeSymbolic {
 };
 
 namespace conic_detail {
+
+// Items whose target is split over several items (.w != 0 on input) get a partial-sum slot each: .w = 1 + slot.  The
+// kernels store such an item's partial sum in its slot and count the finished items of the target; the last one
+// subtracts the target's slots from it in slot order, so the result does not depend on the order in which the items
+// ran.  info[slot] = {target, first slot, end slot of the target, 0}; the first slot also numbers the target's counter.
+inline void number_pieces(std::vector<int> &item, const std::vector<int> &lvl, std::vector<int> &info, int &npart)
+{
+    const int nl = (int)lvl.size() - 1;
+    info.clear();
+    int slot = 0;
+    for (int lv = 0; lv < nl; lv++) {
+        std::vector<std::pair<int, int>> sp;   // (target, item) of the split items of the level
+        for (int w = lvl[lv]; w < lvl[lv + 1]; w++)
+            if (item[4 * (size_t)w + 3]) sp.push_back({item[4 * (size_t)w], w});
+        std::stable_sort(sp.begin(), sp.end(), [](const std::pair<int, int> &x, const std::pair<int, int> &y) { return x.first < y.first; });
+        for (size_t i = 0; i < sp.size();) {
+            const int s0 = slot;
+            size_t j = i;
+            for (; j < sp.size() && sp[j].first == sp[i].first; j++) item[4 * (size_t)sp[j].second + 3] = 1 + slot++;
+            for (int k = s0; k < slot; k++) { info.push_back(sp[i].first); info.push_back(s0); info.push_back(slot); info.push_back(0); }
+            i = j;
+        }
+    }
+    if (info.empty()) info.assign(4, 0);
+    npart = std::max(npart, slot);
+}
 
 inline void transpose_pattern(int nrow, int ncol, const std::vector<int> &rp, const std::vector<int> &ci,
                               std::vector<int> &t_rp, std::vector<int> &t_ri, std::vector<int> &t_vi)
@@ -440,6 +471,7 @@ inline bool cone_symbolic_build(ConeSymbolic &S, int n, int p, int m, const int 
             S.fb_lvl[lv + 1] = (int)(S.fb_item.size() / 4);
         }
         if (S.fa_item.empty()) S.fa_item.assign(4, 0);
+        conic_detail::number_pieces(S.fa_item, S.fa_lvl, S.fc_item, S.npart);
     }
     // ---- supernodal program ----
     {
@@ -581,6 +613,8 @@ inline bool cone_symbolic_build(ConeSymbolic &S, int n, int p, int m, const int 
         };
         build(S.Lr_rp, S.fwp_item, S.fwp_lvl, S.fwp_R);
         build(S.L_cp, S.bwp_item, S.bwp_lvl, S.bwp_R);
+        conic_detail::number_pieces(S.fwp_item, S.fwp_lvl, S.fwc_item, S.npart);
+        conic_detail::number_pieces(S.bwp_item, S.bwp_lvl, S.bwc_item, S.npart);
     }
     return true;
 }
@@ -667,6 +701,7 @@ inline bool cone_symbolic_build_hybrid(ConeSymbolic &S, int cut)
         }
         if (S.hy_fa_item.empty()) S.hy_fa_item.assign(4, 0);
         if (S.hy_fb_item.empty()) S.hy_fb_item.assign(4, 0);
+        conic_detail::number_pieces(S.hy_fa_item, S.hy_fa_lvl, S.hy_fc_item, S.npart);
     }
     // ---- substitutions: (node, entry range) runs per level ----
     {
@@ -684,7 +719,7 @@ inline bool cone_symbolic_build_hybrid(ConeSymbolic &S, int cut)
                 }
                 Rl[lv] = bestR;
                 const int cap = bestR * PF;
-                // a node whose entries end up in more than one item (long run, or several runs) combines them with atomics
+                // a node whose entries end up in more than one item (long run, or several runs) is a split target
                 std::vector<int> nitems(nk, 0);
                 for (const Run &r : runs[lv]) nitems[r.i] += (r.k1 - r.k0 + cap - 1) / cap;
                 for (const Run &r : runs[lv])
@@ -714,6 +749,8 @@ inline bool cone_symbolic_build_hybrid(ConeSymbolic &S, int cut)
         }
         emit(fr, S.hy_fwp_item, S.hy_fwp_lvl, S.hy_fwp_R);
         emit(br, S.hy_bwp_item, S.hy_bwp_lvl, S.hy_bwp_R);
+        conic_detail::number_pieces(S.hy_fwp_item, S.hy_fwp_lvl, S.hy_fwc_item, S.npart);
+        conic_detail::number_pieces(S.hy_bwp_item, S.hy_bwp_lvl, S.hy_bwc_item, S.npart);
     }
     // ---- top supernodes: descriptors in level order, update scatter lists as target ids ----
     {

@@ -3,7 +3,7 @@
 // Replaces discretize!/derivs_foh/set_update_matrices (src/solvers/discretization.jl:160-406)
 // and rk4_generic/rk4_core_step/linterp (src/utils/helper.jl:451-501, 411-424, 107-118).
 //
-// Work decomposition (B200): one warp per (seed b, segment k) -- the B*(N-1) items are
+// Work decomposition: one warp per (seed b, segment k) -- the B*(N-1) items are
 // independent (discretization.jl:182 only reads ref.xd/ud/p).  Inside the warp the augmented
 // propagation vector V = [x; Phi; PB-; PB+; PF; Pr; PE] is laid out COLUMN-PER-LANE:
 //   lanes 0..NX-1      hold the columns of Phi,
@@ -62,9 +62,8 @@ __device__ __forceinline__ double shfl_d(double v, int src)
 // IMP = 1: IMPULSE discretization (discretization.jl:186-193, 304-340, 384-390): the segment starts from the
 // impulse-updated state x_k + f(t_k, -k, x_k, u_k, p), coasts with u = 0, and B_k = A_k * B(t_k, -k, x_k, u_k, p) (one
 // input block: Bm; Bp is written as zero).  Phi, F, r and E columns are the FOH ones evaluated at u = 0.
-// MB: resident 128-thread blocks per SM the register allocation is held to (2: 255 registers, no spills; 3: 168; 4: 128
-// with a few hundred bytes of spills) -- more warps per scheduler to hide the fixed-latency chains of the stage, chosen
-// by measurement (scpb_api.cu: launch_disc)
+// MB: resident 128-thread blocks per SM the register allocation is held to (2: 255 registers; 3: 168; 4: 128, each step
+// with more spill code) -- more warps per scheduler to hide the fixed-latency chains of the stage (scpb_api.cu: launch_disc)
 template <class M, int IMP, int MB = 2>
 __global__ void __launch_bounds__(128, MB) k_discretize_foh(const DiscArgs a)
 {

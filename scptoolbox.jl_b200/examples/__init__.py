@@ -1,1 +1,1 @@
-"""Example problem definitions (mirrors of test/examples/* of the reference) for the B200 path."""
+"""Example problem definitions (mirrors of test/examples/* of the reference) for the GPU path."""

@@ -1,4 +1,4 @@
-"""Double integrator with friction as a free-final-time, minimum-time PTR problem (BASELINE config C1) on the B200 API.
+"""Double integrator with friction as a free-final-time, minimum-time PTR problem (BASELINE config C1) on the GPU API.
 
 The reference ships this plant only as a fixed-time LCvx program (test/examples/double_integrator/definition.jl:38-118
 on parameters.jl:50-64: f = [x2; u - g], travel distance s, two parameter choices).  The SCP form is a NEW definition

@@ -1,4 +1,4 @@
-"""6-DoF free-flyer in the space station as a PTR problem (BASELINE config C5) on the B200 API.
+"""6-DoF free-flyer in the space station as a PTR problem (BASELINE config C5) on the GPU API.
 
 Vehicle, environment and trajectory data: test/examples/freeflyer/parameters.jl:105-190; problem definition:
 test/examples/freeflyer/definition.jl (dims :42-49, scaling advice :52-67, guess :84-167, cost :170-222,

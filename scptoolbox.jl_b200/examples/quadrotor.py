@@ -1,4 +1,4 @@
-"""Quadrotor obstacle avoidance (BASELINE config C4) on the B200 API, in its GuSTO flavour.
+"""Quadrotor obstacle avoidance (BASELINE config C4) on the GPU API, in its GuSTO flavour.
 
 Vehicle, environment and trajectory data: test/examples/quadrotor/parameters.jl:96-135; problem definition:
 test/examples/quadrotor/definition.jl (dims :40-45, scaling advice :47-58, guess :60-91, cost :93-138, dynamics :140-186,

@@ -1,4 +1,4 @@
-"""Mars powered-descent guidance as a free-final-time PTR problem (BASELINE config C2) on the B200 API.
+"""Mars powered-descent guidance as a free-final-time PTR problem (BASELINE config C2) on the GPU API.
 
 The reference ships this vehicle only as a single-shot LCvx program (test/examples/rocket_landing/definition.jl:33-140
 on parameters.jl:78-150); the SCP form is a NEW definition on the same data: state x = [r(3) v(3) z = ln m], input

@@ -1,4 +1,4 @@
-"""Starship landing flip -- mirror of test/examples/starship_flip/{parameters,definition}.jl on the B200 API.
+"""Starship landing flip -- mirror of test/examples/starship_flip/{parameters,definition}.jl on the GPU API.
 
 parameters.jl:100-212 -> StarshipProblem ; definition.jl:29-41 define_problem! ; set_scale! :50-79 ;
 set_cost! :454-478 ; set_dynamics! :552-637 (device pack SCPB_MODEL_STARSHIP) ; set_convex_constraints! :639-702 ;

@@ -1,4 +1,4 @@
-"""GuSTO -- host-side mirror of src/solvers/gusto.jl for the B200 path (pen = :quad).
+"""GuSTO -- host-side mirror of src/solvers/gusto.jl for the GPU path (pen = :quad).
 
   Parameters           gusto.jl:58-85
   create(pars, traj)   gusto.jl:146-205 + the shared SCPProblem machinery (ptr.py)

@@ -384,4 +384,5 @@ def debug_kkt_solve(A, G, l, soc_dims, perm, Avals, Gvals, wm, delta, rhs, delta
                                   pAv, pGv, pwm, float(delta), float(delta_dyn), pr, sol.ctypes.data_as(_dp), info)
     if rc != 0:
         raise ScpbError(f"scpb_debug_kkt_solve failed ({rc})")
-    return sol, dict(nnzL=int(info[0]), levels=int(info[1]), factor_ops=int(info[2]), assembly_ops=int(info[3]))
+    return sol, dict(nnzL=int(info[0]), levels=int(info[1]), factor_ops=int(info[2]), assembly_ops=int(info[3]),
+                     split_items=int(info[4]))

@@ -1,6 +1,6 @@
 """Elimination orderings for the reduced KKT matrix  [dI + G'W^-2G, A'; A, -dI]  of the cone solver.
 
-`stage_order` is the B200-specific choice: optimal-control subproblems are chains of N stages
+`stage_order` is the GPU-specific choice: optimal-control subproblems are chains of N stages
 coupled only through the dynamics rows (discretization.jl:454-465) and a few global parameters, so
   1. every stage's local variables and local equality rows are eliminated first (N independent
      elimination sub-trees -> wide levels for the level-scheduled LDL'),

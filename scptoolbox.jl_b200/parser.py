@@ -1,4 +1,4 @@
-"""Host-side conic 'parser' of the B200 path: the mirror of src/parser/{program,constraint,cone,cost}.jl.
+"""Host-side conic 'parser' of the GPU path: the mirror of src/parser/{program,constraint,cone,cost}.jl.
 
 The reference rebuilds a JuMP model every SCP iteration (ptr.jl:470-478).  Here the subproblem is
 built ONCE, symbolically: a coefficient is not a number but a `Lin` -- a linear combination of

@@ -118,7 +118,7 @@ def problem_set_s(pbm, ns, struct, gcols=None):
 
 
 def problem_advise_parameter_stage(pbm, stage_of):
-    """B200-specific ordering advice: stage_of(N) -> list (len np) with the time node a parameter is tied to, or
+    """GPU-specific ordering advice: stage_of(N) -> list (len np) with the time node a parameter is tied to, or
     -1 for a genuinely global parameter (used only for the elimination order of the KKT factorisation)."""
     pbm.p_stage = stage_of
 

@@ -1,4 +1,4 @@
-"""PTR -- host-side mirror of src/solvers/ptr.jl for the B200 path.
+"""PTR -- host-side mirror of src/solvers/ptr.jl for the GPU path.
 
   Parameters           ptr.jl:57-71
   create(pars, traj)   ptr.jl:148-195 + SCPProblem / compute_scaling (scp.jl:140-157, 376-517)

@@ -1,4 +1,4 @@
-"""SCvx -- host-side mirror of src/solvers/scvx.jl for the B200 path.
+"""SCvx -- host-side mirror of src/solvers/scvx.jl for the GPU path.
 
   Parameters           scvx.jl:57-81
   create(pars, traj)   scvx.jl:160-205 + the shared SCPProblem machinery (ptr.py)

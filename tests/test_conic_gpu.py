@@ -3,7 +3,7 @@
 Tolerances (fp64): objective 1e-6 relative to max(1,|obj|) against HiGHS / the oracle IPM (the solver
 targets ECOS' 1e-8 and returns its best iterate when the fp64 factorisation floors slightly above it),
 primal/dual residuals <= 1e-6 relative, and -- where the optimum is unique (random programs) -- x within
-1e-4 of the oracle solution (measured: 4e-5 worst case).
+1e-4 of the oracle solution.
 """
 import numpy as np
 import pytest

@@ -148,6 +148,9 @@ def test_supernodal_program_on_the_product_template(pkg, monkeypatch):
         assert np.abs(s1 - s3).max() <= 1e-8 * scale, (cut, np.abs(s1 - s3).max())
         assert i3["scalar_levels"] == i1["levels"] and i3["levels"] + i3["top_levels"] <= 0.6 * i1["levels"], (cut, i3)
         assert i3["top_levels"] == i2["sn_levels"] - cut and i3["top_supernodes"] > 0
+    # targets too long for one item are split over several; the interpreter applies their partial sums through the
+    # slots the device uses and rejects a slot numbering that does not cover each split target's items in its level
+    assert i1["split_items"] > 0, i1
 
 
 def test_native_rcm_order(pkg):

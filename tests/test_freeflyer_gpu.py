@@ -77,7 +77,7 @@ def test_freeflyer_ptr_matches_oracle_ptr(pkg, handle):
         ep = np.abs((sol.p[b] - rs.p) / sc.Sp).max()
         dJ = abs(sol.cost[b] - rs.J_aug) / max(1.0, abs(rs.J_aug))
         print("freeflyer parity seed", b, "ex", ex, "eu", eu, "ep", ep, "dJ", dJ)
-        assert dJ <= 1e-6 and max(ex, eu, ep) <= 5e-5      # measured on B200: dJ 8e-7, ex 1.1e-5, eu 3e-6, ep 3e-7 (4 unconverged iterations)
+        assert dJ <= 1e-6 and max(ex, eu, ep) <= 5e-5      # 4 unconverged iterations: the figures are printed above
 
 
 def test_freeflyer_c5_batch(pkg, handle):

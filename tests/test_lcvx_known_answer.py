@@ -141,6 +141,6 @@ def test_cuda_cone_solver_reproduces_the_maximum_principle_solution(pkg, handle)
         # against the oracle's interior point: the same optimum of the same (strictly convex in sigma2, u) program
         print("seed", b, "cost", cost, ref["obj"], "max |u - u_oracle|", np.abs(out["x"][b][iu:iu + N] - ref["z"][iu:iu + N]).max())
         assert abs(cost - ref["obj"]) <= 1e-6 * max(1.0, abs(ref["obj"]))
-        assert np.abs(out["x"][b][iu:iu + N] - ref["z"][iu:iu + N]).max() <= 3e-4   # measured 3.0e-5 / 4.9e-5 (both solvers at 1e-8 / 1e-10)
+        assert np.abs(out["x"][b][iu:iu + N] - ref["z"][iu:iu + N]).max() <= 3e-4   # both solvers at 1e-8 / 1e-10
         # ... and against the analytic optimum
         _check_against_mp(b + 1, out["x"][b], cost, iu, ix, 0.08, 2e-2)
