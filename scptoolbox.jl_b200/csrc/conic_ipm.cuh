@@ -814,27 +814,33 @@ __device__ __forceinline__ void kkt_solve(const IpmProgram &P, Ctx &c, const Ipm
         __syncthreads();
         apply_winv2(P, c, wm, socw, soceta, gm, e1);  // e1: max(n,m)-sized scratch holding W^-2 G dx
         __syncthreads();
-        double nrm[2] = {0.0, 0.0};   // |residual|_inf, |rhs|_inf
+        // |residual|_inf, |rhs|_inf; a NaN entry counts as +inf (fmax would drop it)
+        double nrm[2] = {0.0, 0.0};
         for (int v = c.slot; v < P.n; v += c.nslots) {
             const double r = bx[GI(v)] - col_dot(P.Gt_rp, P.Gt_ri, P.Gt_vi, Gv, e1, v, G, sg) -
                              col_dot(P.At_rp, P.At_ri, P.At_vi, Av, dy, v, G, sg);
             rhs[GI(P.iperm[v])] = r;
-            nrm[0] = fmax(nrm[0], fabs(r)); nrm[1] = fmax(nrm[1], fabs(bx[GI(v)]));
+            nrm[0] = fmax(nrm[0], r == r ? fabs(r) : CUDART_INF); nrm[1] = fmax(nrm[1], fabs(bx[GI(v)]));
         }
         for (int r = c.slot; r < P.p; r += c.nslots) {
             const double rr = by[GI(r)] - row_dot(P.A_rp, P.A_ci, Av, dx, r, G, sg);
             rhs[GI(P.iperm[P.n + r])] = rr;
-            nrm[0] = fmax(nrm[0], fabs(rr)); nrm[1] = fmax(nrm[1], fabs(by[GI(r)]));
+            nrm[0] = fmax(nrm[0], rr == rr ? fabs(rr) : CUDART_INF); nrm[1] = fmax(nrm[1], fabs(by[GI(r)]));
         }
         seed_reduce<2>(c, nrm, 2);   // ends with a barrier: rhs is complete as well
         if (c.tid == 0) {
+            // the group refines again while one of its seeds asks for it.  Finished seeds (converged, failed, skipped by
+            // the caller, padded lanes) have no vote: their directions are not used.  Nor has a seed whose residual is
+            // not finite: refining cannot repair it, and its next residual check ends it as NUMERICAL.  Without these
+            // exclusions a seed's bits depended on whether its group was padded or held a NaN seed.
             int again = 0;
             for (int q = 0; q < G; q++) {
                 const double res = c.out[q], ref = c.out[IPM_MAXG + q];
+                if (c.s_done[q] || !isfinite(res)) continue;
                 // early iterations only need a direction; the last ones (small mu: the scaling matrix spans > 20 orders of
                 // magnitude) need every digit, or the iterates stall a decade or two above the requested gap
                 const double tol_ = (c.s_mu[q] > c.mu_tight) ? c.reftol : fmin(c.reftol, 1e-13);
-                if (!(res <= tol_ * (1.0 + ref))) again = 1;   // NaN counts as "not converged"
+                if (!(res <= tol_ * (1.0 + ref))) again = 1;
             }
             *c.flag = again;
         }

@@ -9,8 +9,12 @@ from tests.test_ptr_gpu import _setup
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.xfail(reason="device path of q_tr = 4 not validated: fails on an H100 (the template is CPU-verified "
-                          "against the oracle's program, tests/test_ptr_template.py)", strict=False)
+@pytest.mark.xfail(reason="the PTR loop with a trust-region norm other than LINF ends 1e-4..1e-3 (ex(phys)) away from "
+                          "the oracle loop after 5 iterations; the cone solves of the q_tr = 4 subproblems match the "
+                          "oracle (test_conic_seeds_gpu.py::test_starship_soc_subproblems_match_the_oracle) and q_tr = 1, "
+                          "which has no second-order cone, deviates the same way (test_ptr_with_soc_trust_regions_"
+                          "matches_the_oracle_loop), so the cause is in the loop, not in the GEOM / SOC cone solve",
+                   strict=False)
 def test_ptr_with_the_squared_two_norm_trust_region(pkg, handle):
     """q_tr = 4 (ptr.jl:582, 604-630: SOC trust-region cones whose radius enters through the GEOM cone): the batched PTR
     against the oracle PTR on the starship problem, 5 forced iterations."""
