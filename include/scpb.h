@@ -36,7 +36,9 @@ enum {
     SCPB_MODEL_FREEFLYER = 5, /* freeflyer/definition.jl:224-284; par: mass, J[9], Jinv[9] (col-major) */
     SCPB_MODEL_RENDEZVOUS2D = 6 /* rendezvous_planar/definition.jl:147-243 (impulsive RCS thrust): x=[r2,v2,theta,omega],
                                  u[0..2]=(f-,f+,f0) of 12 inputs, p=[tdil]; par: m, J, lu, lv, n.  The only pack with
-                                 impulse semantics (the reference's f/B called with a negative segment index) */
+                                 impulse semantics (the reference's f/B called with a negative segment index).
+                                 Its constraint pack (the RCS deadband, definition.jl:337-413: ns = 6, ng = 1) reads
+                                 par[5] = f_db, par[6] = f_max, par[7] = kappa, the sharpness of the smooth OR */
 };
 #define SCPB_MAX_PAR 64
 
@@ -176,6 +178,9 @@ typedef struct {
     int32_t iter_max;
     int32_t ng;              /* packed columns of ds/dp per node (the constraint pack's NG; = np for most packs) */
     double eps_abs, eps_rel, feas_tol;
+    int32_t method;          /* SCPB_FOH (0: a zero-initialised descriptor) or SCPB_IMPULSE (a model pack with impulse
+                                semantics only; the fill matrix W then references no oBp source, state_update!,
+                                discretization.jl:469-494).  scpb_scvx_attach / scpb_gusto_attach refuse IMPULSE. */
 } scpb_ptr_desc;
 
 /* scale = [Sx,Su,Sp | cx,cu,cp | iSx] (diagonals, scp.jl:483-516); t_grid[N]. */
@@ -183,6 +188,12 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
                        const int32_t *W_colind, const double *W_vals, const double *scale, const double *t_grid,
                        scpb_ptr *out);
 int32_t scpb_ptr_free(scpb_ptr s);
+/* Replace the model parameter block (par[npar], same layout as scpb_model_set) that the problem captured at
+ * scpb_ptr_setup; the model, its dimensions and the template stay.  npar must lie between the length of the block given
+ * to scpb_model_set before setup and SCPB_MAX_PAR (SCPB_ERR_ARG otherwise): a shorter block would zero trailing entries.  Later solves use the new block,
+ * e.g. the next step of a homotopy on a constraint-pack parameter (the reference sets mdl.traj.kappa between two
+ * PTR.solve calls on one problem, test/examples/rendezvous_planar/tests.jl:66-78). */
+int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar);
 /* host arrays: initial guesses xd0[B][N][nx], ud0[B][N][nu], p0[B][np]; outputs the final iterates, per-seed
  * status (0 = stopping criterion met, 1 = iter_max reached [the reference still reports SCP_SOLVED],
  * 2+16*cone_status = SCP_FAILED), iteration counts, J_aug, deviation, dynamic feasibility flags and
@@ -245,6 +256,13 @@ int32_t scpb_gusto_solve(scpb_ptr ptr, int32_t B, const double *xd0, const doubl
 /* Measured fp64 FMA throughput of the handle's device in TFLOP/s (a register-resident FMA microkernel, best of 3
  * timed launches): the denominator of the discretization kernel's roofline in bench.py. */
 int32_t scpb_debug_fp64_peak(scpb_handle h, double *tflops);
+
+/* Test hook: the nonconvex-constraint pack of the selected model (scpb_model_set) evaluated on the device at every seed
+ * and node, as the PTR loop's linearisation evaluates it: t_grid[N], xd[B][N][nx], ud[B][N][nu], p[B][np] -> s[B][N][ns],
+ * C[B][N][ns*nx], D[B][N][ns*nu], G[B][N][ns*ng] (row-major; G packed, see scpb_ptr_desc.ng).  ns / ng must be the pack's. */
+int32_t scpb_debug_constraints(scpb_handle h, int32_t B, int32_t N, int32_t ns, int32_t ng, const double *t_grid,
+                               const double *xd, const double *ud, const double *p, double *s, double *C, double *D,
+                               double *G);
 
 /* Diagnostic: per-level cycle counters of CTA 0 in the last scpb_cone_solve / scpb_ptr_solve launch, recorded
  * only when the environment variable SCPB_LEVEL_PROFILE is set: out[0..L) numeric factorisation, out[L..2L)

@@ -101,7 +101,8 @@ function scvx_solve(h::Handle, ptr, B, xd0, ud0, p0, opts::ConeOpts, xd, ud, p, 
 end
 
 # scpb_ptr_setup / scpb_ptr_solve / scpb_ptr_free (PTR.solve for a batch, src/solvers/ptr.jl:448-532).  The descriptor
-# mirrors scpb_ptr_desc field by field (28 Int32 + 3 Float64; Julia lays isbits structs out like C).
+# mirrors scpb_ptr_desc field by field (28 Int32 + 3 Float64 + 1 Int32; Julia lays isbits structs out like C).
+# method: 0 = FOH, 1 = IMPULSE (PTR only, a model pack with impulse semantics).
 struct PtrDesc
     N::Int32; Nsub::Int32; nx::Int32; nu::Int32; np::Int32; ns::Int32; nf::Int32
     nsrc::Int32; oA::Int32; oBm::Int32; oBp::Int32; oF::Int32; or_::Int32; oE::Int32; oC::Int32; oD::Int32; oG::Int32
@@ -109,6 +110,7 @@ struct PtrDesc
     nval::Int32; vx::Int32; vu::Int32; vp::Int32
     q_exit::Int32; iter_max::Int32; ng::Int32
     eps_abs::Float64; eps_rel::Float64; feas_tol::Float64
+    method::Int32
 end
 
 function ptr_setup(h::Handle, cone, desc::PtrDesc, W_rp::Vector{Int32}, W_ci::Vector{Int32}, W_v::Vector{Float64},
@@ -131,6 +133,12 @@ function ptr_solve(h::Handle, ptr, B, xd0, ud0, p0, opts::ConeOpts, xd, ud, p, s
 end
 
 ptr_free(ptr) = ccall((:scpb_ptr_free, libscpb), Int32, (Ptr{Cvoid},), ptr)
+
+# scpb_ptr_set_par: the model parameter block for the next ptr_solve calls of this problem, e.g. after
+# `mdl.traj.κ = hom_κ(x)` between two solves of a homotopy (test/examples/rendezvous_planar/tests.jl:66-78)
+ptr_set_par(h::Handle, ptr, par::Vector{Float64}) =
+    check(h, ccall((:scpb_ptr_set_par, libscpb), Int32, (Ptr{Cvoid}, Ptr{Float64}, Int32), ptr, par, length(par)),
+          "scpb_ptr_set_par")
 
 # scpb_gusto_attach / scpb_gusto_solve (GuSTO.solve for a batch, src/solvers/gusto.jl:425-502, pen = :quad)
 struct GustoDesc

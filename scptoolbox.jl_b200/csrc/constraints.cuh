@@ -125,3 +125,57 @@ struct Constr<SCPB_MODEL_FREEFLYER> {
         for (int j = 0; j < NISS; j++) G[3 * NG + j] = -(exp(hom * dl[j] - a) / E);
     }
 };
+
+// rendezvous_planar/definition.jl:337-413: the RCS deadband.  For thruster i, with the smooth OR of the predicates
+// "reference thrust above / below the deadband",
+//   s_2i = f_i - OR(fr_i) fr_i,   s_2i+1 = OR(fr_i) fr_i - f_i,   D = +-1 on f_i, -+(dOR/dfr fr_i + OR) on fr_i.
+// OR = or(...; kappa, match, normalize) -> indicator -> sigmoid -> logsumexp (src/utils/helper.jl:623-807).  Every step
+// keeps the reference's operation order, with no contraction into fma: at the sharp end of the homotopy
+// (kappa ~ 4.6e3) sigma = 1 - 1/(1 + exp(kappa L)) rounds to exactly 1 and the gradient factor
+// c = exp(kappa L + 2 log(1 - sigma)) to exactly 0, and a rearranged formula would not saturate on the same inputs.
+// par: m, J, lu, lv, n (dynamics pack) [0..4], then f_db [5], f_max [6], kappa [7].
+template <>
+struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
+    static constexpr int NS = 6, NX = 6, NU = 12, NG = 1;
+    __device__ static constexpr int gcol(int, int j) { return j; }
+    // sigmoid([f0, f1], [g0, g1]; kappa) of two scalar predicates with scalar gradients: value sg, gradient dsg
+    __device__ __forceinline__ static void sigmoid2(double f0, double f1, double g0, double g1, double kap, double &sg,
+                                                    double &dsg)
+    {
+        const double a = fmax(__dmul_rn(kap, f0), __dmul_rn(kap, f1));
+        const double e0 = exp(__dsub_rn(__dmul_rn(kap, f0), a)), e1 = exp(__dsub_rn(__dmul_rn(kap, f1), a));
+        const double E = __dadd_rn(e0, e1);
+        const double L = __ddiv_rn(__dadd_rn(a, log(E)), kap);
+        const double kL = __dmul_rn(kap, L);
+        sg = __dsub_rn(1.0, __ddiv_rn(1.0, __dadd_rn(1.0, exp(kL))));
+        const double dL = __dadd_rn(__dmul_rn(g0, __ddiv_rn(e0, E)), __dmul_rn(g1, __ddiv_rn(e1, E)));
+        const double c = exp(__dadd_rn(kL, __dmul_rn(2.0, log(__dsub_rn(1.0, sg)))));
+        dsg = __dmul_rn(__dmul_rn(kap, c), dL);
+    }
+    __device__ static void eval(const ModelPar &P, double, int, int, const double *, const double *u, const double *,
+                                double *s, double *C, double *D, double *G)
+    {
+        const double fdb = P.v[5], fmx = P.v[6], kap = P.v[7];
+        const double nrm = __dadd_rn(fmx, fdb);
+        for (int i = 0; i < NS * NX; i++) C[i] = 0.0;
+        for (int i = 0; i < NS * NU; i++) D[i] = 0.0;
+        for (int i = 0; i < NS * NG; i++) G[i] = 0.0;
+        double off, unused;   // indicator's y-shift: the OR is exact at the predicates' values `match`
+        sigmoid2(__ddiv_rn(__dsub_rn(fmx, fdb), nrm), __ddiv_rn(__dsub_rn(-fdb, fmx), nrm), 0.0, 0.0, kap, off, unused);
+        const double shift = __dsub_rn(1.0, off);
+        for (int i = 0; i < 3; i++) {
+            const double f = u[i], fr = u[3 + i];
+            double sg, dOR;
+            sigmoid2(__ddiv_rn(__dsub_rn(fr, fdb), nrm), __ddiv_rn(__dsub_rn(-fdb, fr), nrm), __ddiv_rn(1.0, nrm),
+                     __ddiv_rn(-1.0, nrm), kap, sg, dOR);
+            const double OR = __dadd_rn(sg, shift), ORfr = __dmul_rn(OR, fr);
+            const double dORfr = __dadd_rn(__dmul_rn(dOR, fr), OR);
+            s[2 * i] = __dsub_rn(f, ORfr);
+            s[2 * i + 1] = __dsub_rn(ORfr, f);
+            D[(2 * i) * NU + i] = 1.0;
+            D[(2 * i) * NU + 3 + i] = -dORfr;
+            D[(2 * i + 1) * NU + i] = -1.0;
+            D[(2 * i + 1) * NU + 3 + i] = dORfr;
+        }
+    }
+};

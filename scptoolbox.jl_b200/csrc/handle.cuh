@@ -20,6 +20,7 @@ struct scpb_handle_s {
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int model_id = 0, nx = 0, nu = 0, np = 0;
     ModelPar par{};
+    int npar = 0;              // entries of par the caller gave (scpb_model_set); the rest are zero
     long long launches = 0;
     char err[512] = {0};
     int *d_status = nullptr;

@@ -214,6 +214,7 @@ struct scpb_ptr_s {
     scpb_cone_s *cone = nullptr;
     int model_id = 0;            // dynamics pack and parameters captured at setup: a later scpb_model_set on the same
     ModelPar par{};              // handle (another problem sharing it) must not change what THIS problem solves
+    int npar = 0;                // length of that block: scpb_ptr_set_par refuses a shorter one
     scpb_ptr_desc d{};
     std::vector<void *> dev;
     int *W_rp = nullptr, *W_ci = nullptr;
@@ -375,7 +376,7 @@ static int run_discretize(scpb_ptr_s *s, int B, int G, const double *xd, const d
     a.E = grouped(sb, G, d.nsrc, d.oE, nx * nx);
     OutView df{}; df.ptr = s->defect; df.Gq = 1; df.sGrp = (long long)(d.N - 1) * nx; df.sB = 0; df.sK = nx; df.sE = 1;
     a.defect = df;
-    return scpb_internal_discretize(s->h, a, d.feas_tol, s->feas, SCPB_FOH, st);
+    return scpb_internal_discretize(s->h, a, d.feas_tol, s->feas, d.method, st);
 }
 
 
@@ -698,7 +699,56 @@ static void launch_linearize(scpb_ptr_s *s, const PtrDev &pd, int nbn, cudaStrea
     if (has && s->model_id == SCPB_MODEL_STARSHIP) k_linearize<Constr<SCPB_MODEL_STARSHIP>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
     else if (has && s->model_id == SCPB_MODEL_FREEFLYER) k_linearize<Constr<SCPB_MODEL_FREEFLYER>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
     else if (has && s->model_id == SCPB_MODEL_QUADROTOR) k_linearize<Constr<SCPB_MODEL_QUADROTOR>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
+    else if (has && s->model_id == SCPB_MODEL_RENDEZVOUS2D)
+        k_linearize<Constr<SCPB_MODEL_RENDEZVOUS2D>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
     else k_linearize<Constr<0>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
+}
+
+// scpb_debug_constraints: the pack's s, C, D, G at every (seed, node), one thread each
+template <class CP>
+__global__ void k_debug_constr(const ModelPar par, int B, int N, const double *t_grid, const double *xd, const double *ud,
+                               const double *p, int np, double *s, double *C, double *D, double *G)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)B * N) return;
+    const int b = (int)(i / N), k = (int)(i % N);
+    constexpr int NS = CP::NS, NX = CP::NX, NU = CP::NU, NG = CP::NG;
+    CP::eval(par, t_grid[k], N, k, xd + (size_t)i * NX, ud + (size_t)i * NU, p + (size_t)b * np, s + (size_t)i * NS,
+             C + (size_t)i * NS * NX, D + (size_t)i * NS * NU, G + (size_t)i * NS * NG);
+}
+
+template <class CP>
+static int debug_constr_t(scpb_handle_s *h, int B, int N, int ns, int ng, const double *t_grid, const double *xd,
+                          const double *ud, const double *p, double *s, double *C, double *D, double *G)
+{
+    constexpr int NS = CP::NS, NX = CP::NX, NU = CP::NU, NG = CP::NG;
+    if (ns != NS || ng != NG || h->nx != NX || h->nu != NU)
+        return set_err(h, SCPB_ERR_ARG, "debug_constraints: the pack has ns=%d, ng=%d, nx=%d, nu=%d", NS, NG, NX, NU);
+    const size_t BN = (size_t)B * N;
+    const size_t n_in[4] = {(size_t)N, BN * NX, BN * NU, (size_t)B * h->np};
+    const size_t n_out[4] = {BN * NS, BN * NS * NX, BN * NS * NU, BN * NS * NG};
+    const double *hin[4] = {t_grid, xd, ud, p};
+    double *hout[4] = {s, C, D, G};
+    double *din[4] = {}, *dout[4] = {};
+    int rc = SCPB_OK;
+    for (int j = 0; j < 4 && rc == SCPB_OK; j++) {
+        if (cudaMalloc(&din[j], sizeof(double) * (n_in[j] + 1)) != cudaSuccess ||
+            cudaMalloc(&dout[j], sizeof(double) * (n_out[j] + 1)) != cudaSuccess ||
+            cudaMemcpyAsync(din[j], hin[j], sizeof(double) * n_in[j], cudaMemcpyHostToDevice, h->stream) != cudaSuccess)
+            rc = set_err(h, SCPB_ERR_CUDA, "debug_constraints: device allocation or copy failed");
+    }
+    if (rc == SCPB_OK) {
+        k_debug_constr<CP><<<(unsigned)((BN + 127) / 128), 128, 0, h->stream>>>(h->par, B, N, din[0], din[1], din[2], din[3],
+                                                                                 h->np, dout[0], dout[1], dout[2], dout[3]);
+        h->launches++;
+        for (int j = 0; j < 4 && rc == SCPB_OK; j++)
+            if (cudaMemcpyAsync(hout[j], dout[j], sizeof(double) * n_out[j], cudaMemcpyDeviceToHost, h->stream) != cudaSuccess)
+                rc = set_err(h, SCPB_ERR_CUDA, "debug_constraints: %s", cudaGetErrorString(cudaGetLastError()));
+        if (cudaStreamSynchronize(h->stream) != cudaSuccess && rc == SCPB_OK)
+            rc = set_err(h, SCPB_ERR_CUDA, "debug_constraints: %s", cudaGetErrorString(cudaGetLastError()));
+    }
+    for (int j = 0; j < 4; j++) { if (din[j]) cudaFree(din[j]); if (dout[j]) cudaFree(dout[j]); }
+    return rc;
 }
 
 template <class M, class CP>
@@ -751,6 +801,8 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
         case SCPB_MODEL_STARSHIP: pns = Constr<SCPB_MODEL_STARSHIP>::NS; png = Constr<SCPB_MODEL_STARSHIP>::NG; break;
         case SCPB_MODEL_QUADROTOR: pns = Constr<SCPB_MODEL_QUADROTOR>::NS; png = Constr<SCPB_MODEL_QUADROTOR>::NG; break;
         case SCPB_MODEL_FREEFLYER: pns = Constr<SCPB_MODEL_FREEFLYER>::NS; png = Constr<SCPB_MODEL_FREEFLYER>::NG; break;
+        case SCPB_MODEL_RENDEZVOUS2D:
+            pns = Constr<SCPB_MODEL_RENDEZVOUS2D>::NS; png = Constr<SCPB_MODEL_RENDEZVOUS2D>::NG; break;
         default: break;
         }
         if (pns != desc->ns || png != desc->ng)
@@ -759,11 +811,17 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
         if (h->model_id == SCPB_MODEL_FREEFLYER && desc->np != 1 + Constr<SCPB_MODEL_FREEFLYER>::NISS * desc->N)
             return set_err(h, SCPB_ERR_ARG, "ptr_setup: the free-flyer pack expects np = 1 + 6 N");
     }
+    if (desc->method != SCPB_FOH && desc->method != SCPB_IMPULSE)
+        return set_err(h, SCPB_ERR_ARG, "ptr_setup: unknown discretization method %d", desc->method);
+    // refused here rather than at the first discretize! of a solve: only the rendezvous pack has impulse semantics
+    if (desc->method == SCPB_IMPULSE && h->model_id != SCPB_MODEL_RENDEZVOUS2D)
+        return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_setup: model %d has no impulse semantics (IMPULSE discretization)",
+                       h->model_id);
     SCPB_CUDA(h, cudaSetDevice(h->device));
     scpb_ptr_s *s = new (std::nothrow) scpb_ptr_s();
     if (!s) return SCPB_ERR_CUDA;
     s->h = h; s->cone = cone; s->d = *desc;
-    s->model_id = h->model_id; s->par = h->par;
+    s->model_id = h->model_id; s->par = h->par; s->npar = h->npar;
     const int nnzW = W_rowptr[desc->nval];
     s->W_rp = up(s, W_rowptr, (size_t)desc->nval + 1);
     s->W_ci = up(s, W_colind, (size_t)nnzW);
@@ -774,6 +832,41 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
     for (void *q : s->dev)
         if (!q) { scpb_ptr_free(s); return set_err(h, SCPB_ERR_CUDA, "ptr_setup: device allocation failed"); }
     *out = s;
+    return SCPB_OK;
+}
+
+int32_t scpb_debug_constraints(scpb_handle h, int32_t B, int32_t N, int32_t ns, int32_t ng, const double *t_grid,
+                               const double *xd, const double *ud, const double *p, double *s, double *C, double *D,
+                               double *G)
+{
+    if (!h) return SCPB_ERR_ARG;
+    if (B <= 0 || N <= 0 || !t_grid || !xd || !ud || !p || !s || !C || !D || !G)
+        return set_err(h, SCPB_ERR_ARG, "debug_constraints: bad arguments");
+    SCPB_CUDA(h, cudaSetDevice(h->device));
+    switch (h->model_id) {
+    case SCPB_MODEL_STARSHIP: return debug_constr_t<Constr<SCPB_MODEL_STARSHIP>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
+    case SCPB_MODEL_QUADROTOR: return debug_constr_t<Constr<SCPB_MODEL_QUADROTOR>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
+    case SCPB_MODEL_FREEFLYER: return debug_constr_t<Constr<SCPB_MODEL_FREEFLYER>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
+    case SCPB_MODEL_RENDEZVOUS2D:
+        return debug_constr_t<Constr<SCPB_MODEL_RENDEZVOUS2D>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
+    default: return set_err(h, SCPB_ERR_UNSUPPORTED, "debug_constraints: model %d has no constraint pack", h->model_id);
+    }
+}
+
+int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar)
+{
+    if (!s) return SCPB_ERR_ARG;
+    if (!par || npar < 1 || npar > SCPB_MAX_PAR)
+        return set_err(s->h, SCPB_ERR_ARG, "ptr_set_par: npar = %d outside 1..%d", npar, SCPB_MAX_PAR);
+    // a shorter block would zero the trailing entries, e.g. the constraint pack's parameters after the dynamics ones
+    if (npar < s->npar)
+        return set_err(s->h, SCPB_ERR_ARG, "ptr_set_par: npar = %d is shorter than the %d entries given at setup", npar,
+                       s->npar);
+    // the kernels of a solve receive the block by value at launch, so an earlier solve that is still queued on the
+    // stream keeps the parameters it was launched with
+    ModelPar q{};
+    for (int i = 0; i < npar; i++) q.v[i] = par[i];
+    s->par = q;
     return SCPB_OK;
 }
 
@@ -1007,6 +1100,7 @@ int32_t scpb_scvx_attach(scpb_ptr s, const scpb_scvx_desc *desc, const int32_t *
     scpb_handle_s *h = s->h;
     if (!desc || !Q_rowptr || !Q_colind || !Q_vals || !Q_const) return set_err(h, SCPB_ERR_ARG, "scvx_attach: null pointer");
     const scpb_ptr_desc &d = s->d;
+    if (d.method != SCPB_FOH) return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: SCvx runs with FOH discretization only");
     if (desc->oeta <= 0 || desc->oeta >= d.nsrc || desc->n_ic < 0 || desc->n_tc < 0)
         return set_err(h, SCPB_ERR_ARG, "scvx_attach: bad descriptor (oeta=%d)", desc->oeta);
     const int nq = 1 + desc->n_ic + desc->n_tc, nnz = Q_rowptr[nq];
@@ -1186,6 +1280,7 @@ int32_t scpb_gusto_attach(scpb_ptr s, const scpb_gusto_desc *desc, const int32_t
     if (!desc || !Q_rowptr || !Q_colind || !Q_vals || !Q_const || (desc->nsq > 0 && !Q_weight))
         return set_err(h, SCPB_ERR_ARG, "gusto_attach: null pointer");
     const scpb_ptr_desc &d = s->d;
+    if (d.method != SCPB_FOH) return set_err(h, SCPB_ERR_UNSUPPORTED, "gusto_attach: GuSTO runs with FOH discretization only");
     if (desc->oeta <= 0 || desc->oeta >= d.nsrc || desc->olam <= 0 || desc->olam >= d.nsrc || desc->olam == desc->oeta ||
         desc->nsq < 0 || desc->q_tr < 0 || desc->q_tr > 2)
         return set_err(h, SCPB_ERR_ARG, "gusto_attach: bad descriptor (oeta=%d, olam=%d, nsq=%d, q_tr=%d)", desc->oeta, desc->olam,

@@ -93,7 +93,7 @@ static void julia_views(DiscArgs &a, int nx, int nu, int np, double *A, double *
 
 extern "C" {
 
-int32_t scpb_version(void) { return 100; }
+int32_t scpb_version(void) { return 101; }
 
 int32_t scpb_create(int32_t device, scpb_handle *out)
 {
@@ -174,6 +174,7 @@ int32_t scpb_model_set(scpb_handle h, int32_t model_id, const double *par, int32
     h->nx = nx; h->nu = nu; h->np = np;
     memset(&h->par, 0, sizeof h->par);
     for (int i = 0; i < npar; i++) h->par.v[i] = par[i];
+    h->npar = npar;
     return SCPB_OK;
 }
 

@@ -49,6 +49,7 @@ SIGNATURES = {
                                     _dp, _dp, _dp, _dp, _dp, _dp, _ip, _ip, _dp]),
     "scpb_ptr_setup": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_void_p)]),
     "scpb_ptr_free": (C.c_int32, [C.c_void_p]),
+    "scpb_ptr_set_par": (C.c_int32, [C.c_void_p, _dp, C.c_int32]),
     "scpb_ptr_solve": (C.c_int32, [C.c_void_p, C.c_int32, _dp, _dp, _dp, C.c_void_p, _dp, _dp, _dp, _ip, _ip,
                                    _dp, _dp, _ip, _dp]),
     "scpb_scvx_attach": (C.c_int32, [C.c_void_p, C.c_void_p, _ip, _ip, _dp, _dp]),
@@ -67,6 +68,8 @@ SIGNATURES = {
                                          _ip, _ip, _dp, _dp, _dp, C.c_double, C.c_double, C.c_int32, _dp, _dp,
                                          C.POINTER(C.c_int64)]),
     "scpb_debug_fp64_peak": (C.c_int32, [C.c_void_p, _dp]),
+    "scpb_debug_constraints": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _dp, _dp, _dp, _dp,
+                                           _dp, _dp, _dp, _dp]),
     "scpb_debug_kkt_solve_dev": (C.c_int32, [C.c_void_p, C.c_int32, _dp, _dp, _dp, C.c_double, _dp, _dp, _ip]),
     "scpb_debug_kkt_new": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, _ip, _ip, _ip, _ip, C.c_int32, C.c_int32, _ip, _ip,
                                        C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
@@ -86,7 +89,8 @@ class PtrDesc(C.Structure):
     _fields_ = [(k, C.c_int32) for k in
                 ("N", "Nsub", "nx", "nu", "np", "ns", "nf", "nsrc", "oA", "oBm", "oBp", "oF", "or_", "oE", "oC", "oD",
                  "oG", "ors", "oxh", "ouh", "oph", "nval", "vx", "vu", "vp", "q_exit", "iter_max", "ng")] + \
-               [(k, C.c_double) for k in ("eps_abs", "eps_rel", "feas_tol")]
+               [(k, C.c_double) for k in ("eps_abs", "eps_rel", "feas_tol")] + \
+               [("method", C.c_int32)]       # FOH / IMPULSE; appended last, so a zero-initialised descriptor means FOH
 
 
 class ScvxDesc(C.Structure):        # scpb_scvx_desc (include/scpb.h)
@@ -240,6 +244,22 @@ class Handle:
         v = C.c_double(0.0)
         self._check(self.lib.scpb_debug_fp64_peak(self.h, C.byref(v)), "scpb_debug_fp64_peak")
         return v.value
+
+    def debug_constraints(self, t_grid, xd, ud, p, ns, ng):
+        """Test hook (scpb_debug_constraints): the selected model's constraint pack at every seed and node.
+        Returns s (B, N, ns), C (B, N, ns, nx), D (B, N, ns, nu), G (B, N, ns, ng)."""
+        xd, pxd = _f64(xd)
+        ud, pud = _f64(ud)
+        p, pp = _f64(p)
+        tg, ptg = _f64(t_grid)
+        B, N = xd.shape[0], xd.shape[1]
+        assert xd.shape == (B, N, self.nx) and ud.shape == (B, N, self.nu) and p.shape == (B, self.np)
+        out = dict(s=np.empty((B, N, ns)), C=np.empty((B, N, ns, self.nx)), D=np.empty((B, N, ns, self.nu)),
+                   G=np.empty((B, N, ns, ng)))
+        g = lambda k: out[k].ctypes.data_as(_dp)
+        rc = self.lib.scpb_debug_constraints(self.h, B, N, ns, ng, ptg, pxd, pud, pp, g("s"), g("C"), g("D"), g("G"))
+        self._check(rc, "scpb_debug_constraints")
+        return out
 
     def discretize_dev(self, t_grid, xd, ud, p, iSx_diag, feas_tol, Nsub, A, Bm, Bp, F, r, E, defect, feas,
                        B, N, method=FOH):

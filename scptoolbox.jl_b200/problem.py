@@ -76,15 +76,22 @@ def problem_set_running_cost(pbm, SGamma, algo="ptr"):
 
 def problem_set_dynamics(pbm, model_id, par, fcols=(0,), A_struct=None, B_struct=None):
     """problem_set_dynamics! (problem.jl:425-450): selects the device pack that evaluates f, A, B, F.
+    par: the pack's parameter block, or a callable returning it, evaluated at every solve and propagate (the reference's
+    closures read the model when they are called, so a model parameter changed between two solves takes effect).
     fcols: parameter index of each active (time-dilation) column of F.
     A_struct / B_struct: optional structural non-zero patterns of df/dx (nx x nx) and df/du (nx x nu); the
     discrete-time blocks inherit the reachability closure (Phi = closure(I + A), B_k = Phi*B, E_k ~ Phi), which
     removes structurally zero coefficients from the dynamics rows of the subproblem."""
     pbm.model_id = int(model_id)
-    pbm.model_par = np.asarray(par, dtype=np.float64)
+    pbm.model_par = par if callable(par) else np.asarray(par, dtype=np.float64)
     pbm.fcols = list(fcols)
     pbm.A_struct = None if A_struct is None else np.asarray(A_struct, bool)
     pbm.B_struct = None if B_struct is None else np.asarray(B_struct, bool)
+
+
+def model_parameters(pbm):
+    """the current parameter block of the device packs (problem_set_dynamics)"""
+    return np.asarray(pbm.model_par() if callable(pbm.model_par) else pbm.model_par, dtype=np.float64)
 
 
 def dltv_masks(pbm):

@@ -19,8 +19,10 @@ import numpy as np
 
 from . import lib, ordering
 from .parser import ConicTemplate, Expr, Lin, matvec
+from .problem import model_parameters
 
-FOH = lib.FOH
+FOH, IMPULSE = lib.FOH, lib.IMPULSE
+IMPULSE_MODELS = (lib.MODEL_RENDEZVOUS2D,)     # device packs with impulse semantics (csrc/models.cuh)
 
 
 @dataclass
@@ -187,9 +189,14 @@ class SCPProblem:
         self.algo = algo
         self.t = t_grid(pars.N)
         traj.scp = pars
+        if pars.disc_method not in (FOH, IMPULSE):
+            raise lib.ScpbError(f"unknown discretization method {pars.disc_method}")
+        if pars.disc_method == IMPULSE and algo != "ptr":
+            raise lib.ScpbError(f"IMPULSE discretization is implemented for PTR only, not for {algo}")
+        if pars.disc_method == IMPULSE and traj.model_id not in IMPULSE_MODELS:
+            raise lib.ScpbError(f"IMPULSE discretization needs a model pack with impulse semantics (model {traj.model_id} "
+                                "has none)")
         self.scale = SCPScaling(traj, handle, self.t)
-        if pars.disc_method != FOH:
-            raise lib.ScpbError("only FOH discretization is implemented on the device")
         self._build()
 
     # ------------------------------------------------------------------ template (ptr.jl:213-293, 565-895)
@@ -215,18 +222,23 @@ class SCPProblem:
         else:                   # scvx.jl:263-264: the penalty epigraph variables are created with the subproblem
             P = prg.new_variable(N, "P", stage="idx")
             Pf = prg.new_variable(2, "Pf", stage=None)
-        # add_dynamics! / state_update! (discretization.jl:424-497)
+        # add_dynamics! / state_update! (discretization.jl:424-497).  IMPULSE (:469-494): one input block, no u_{k+1}
+        # term; u_N stays a variable of the cost, U and the trust region
         from .problem import dltv_masks
         mA, mB, mE = dltv_masks(traj)
+        impulse = pars.disc_method == IMPULSE
         for k in range(N - 1):
             A = sm.mat(sm.oA, k, nx, nx, mask=mA)
             Bm = sm.mat(sm.oBm, k, nx, nu, mask=mB)
-            Bp = sm.mat(sm.oBp, k, nx, nu, mask=mB)
             E = sm.mat(sm.oE, k, nx, nx, mask=mE)
             r = sm.vec(sm.or_, k, nx)
             Fp = sm.mat(sm.oF, k, nx, nf)
-            rhs = [a + b + c + d for a, b, c, d in zip(matvec(A, x[:, k]), matvec(Bm, u[:, k]),
-                                                       matvec(Bp, u[:, k + 1]), matvec(E, vd[:, k]))]
+            if impulse:
+                rhs = [a + b + d for a, b, d in zip(matvec(A, x[:, k]), matvec(Bm, u[:, k]), matvec(E, vd[:, k]))]
+            else:
+                Bp = sm.mat(sm.oBp, k, nx, nu, mask=mB)
+                rhs = [a + b + c + d for a, b, c, d in zip(matvec(A, x[:, k]), matvec(Bm, u[:, k]),
+                                                           matvec(Bp, u[:, k + 1]), matvec(E, vd[:, k]))]
             Fpv = matvec(Fp, [p[j] for j in traj.fcols])
             prg.zero([x[i, k + 1] - (rhs[i] + Fpv[i] + Expr(None, r[i])) for i in range(nx)], "dynamics")
         # convex state / input constraints (scp.jl:685-734)
@@ -354,7 +366,7 @@ class SCPProblem:
         self.nval = self.W.shape[0]
         # ---- device objects ----
         h = self.handle
-        h.model_set(traj.model_id, traj.model_par, nx, nu, np_)
+        h.model_set(traj.model_id, model_parameters(traj), nx, nu, np_)
         self.perm = ordering.stage_order(cp["A"], cp["G"], cp["var_stage"], N)
         self.cone = lib.ConeProblem(h, cp["A"], cp["G"], cp["l"], cp["soc_dims"], perm=self.perm)
         d = lib.PtrDesc()
@@ -367,6 +379,7 @@ class SCPProblem:
         d.q_exit = {np.inf: 0, 1: 1, 2: 2}[pars.q_exit]
         d.iter_max = pars.iter_max
         d.eps_abs, d.eps_rel, d.feas_tol = pars.eps_abs, pars.eps_rel, pars.feas_tol
+        d.method = pars.disc_method
         self.desc = d
         scale = np.concatenate([sc.Sx, sc.Su, sc.Sp, sc.cx, sc.cu, sc.cp, 1.0 / sc.Sx])
         self._keep = [np.ascontiguousarray(self.W.indptr, dtype=np.int32),
@@ -412,10 +425,19 @@ def create(pars: Parameters, traj, handle, l1_block=4) -> SCPProblem:
     return SCPProblem(pars, traj, handle, l1_block=l1_block)
 
 
+def set_parameters(pbm: SCPProblem, par=None):
+    """Replace the model parameter block the device problem uses (scpb_ptr_set_par); None: the model's current block."""
+    par, pp = lib._f64(model_parameters(pbm.traj) if par is None else par)
+    pbm.handle._check(pbm.handle.lib.scpb_ptr_set_par(pbm.ptr, pp, par.size), "scpb_ptr_set_par")
+
+
 def solve(pbm: SCPProblem, guesses=None, **cone_opts) -> SCPBatchSolution:
     """PTR.solve (ptr.jl:448-532) for a batch: guesses = (xd0 (B,N,nx), ud0 (B,N,nu), p0 (B,np));
-    None => the problem's own guess (one seed)."""
+    None => the problem's own guess (one seed).  The model's parameter block is read again here, as the reference's
+    closures read the model at call time: a parameter changed between two solves (a homotopy step) takes effect
+    without a new create."""
     traj, pars, h = pbm.traj, pbm.pars, pbm.handle
+    set_parameters(pbm)
     if guesses is None:
         x0, u0, p0 = traj.guess(pars.N)
         guesses = (x0[None], u0[None], p0[None])
@@ -518,7 +540,7 @@ def propagate(pbm: SCPProblem, sol: SCPBatchSolution, res=None) -> SCPBatchSolut
     trajectories; here failed seeds are propagated as well (their xc is simply not meaningful)."""
     pars = pbm.pars
     res = int(res) if res is not None else 2 * pars.Nsub * (pars.N - 1)
-    pbm.handle.model_set(pbm.traj.model_id, pbm.traj.model_par, pbm.traj.nx, pbm.traj.nu, pbm.traj.np)
-    sol.tc, sol.xc, sec = pbm.handle.propagate(pbm.t, sol.xd, sol.ud, sol.p, res)
+    pbm.handle.model_set(pbm.traj.model_id, model_parameters(pbm.traj), pbm.traj.nx, pbm.traj.nu, pbm.traj.np)
+    sol.tc, sol.xc, sec = pbm.handle.propagate(pbm.t, sol.xd, sol.ud, sol.p, res, method=pars.disc_method)
     sol.timing["propagate"] = sec
     return sol
