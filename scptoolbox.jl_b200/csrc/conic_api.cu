@@ -174,6 +174,17 @@ int scpb_internal_cone_run(scpb_cone_s *c, const IpmOpts &o, const int *skip, cu
     // shared-memory substitution vector like the supernodal variant
     const bool hy = c->hy_ok && c->D.vsmem && !c->D.sn;
     const IpmProgram &Pl = hy ? c->P_hy : c->P;
+    // partial sums of the split targets of one level: the factorisation's slots share the window of the substitution
+    // vector (it is free while the factorisation runs), the substitutions' slots and counters follow it; global memory
+    // when that does not fit or the vector itself is not in shared memory
+    {
+        const size_t G = (size_t)c->D.G;
+        const size_t win = sizeof(double) * std::max<size_t>((size_t)c->S.nk, (size_t)Pl.npf) * G;
+        const size_t sbytes = (sizeof(double) + sizeof(unsigned)) * (size_t)Pl.nps * G;
+        c->D.psmem = (c->D.vsmem && !c->D.sn && smem - vbytes + win + sbytes <= 200 * 1024 &&
+                      !getenv("SCPB_GLOBAL_SLOTS")) ? 1 : 0;   // env: force the global slots (tests)
+        if (c->D.psmem) smem += win - vbytes + sbytes;
+    }
     c->hy_used = hy ? c->S.hy_cut : 0;
     c->D.lvl_prof = (c->d_prof && getenv("SCPB_LEVEL_PROFILE")) ? 1 : 0;   // diagnostic: per-level cycle counters of CTA 0
     if (hy && c->S.hy_nlevels + c->S.hy_ntl > c->S.nlevels) c->D.lvl_prof = 0;   // the counters are sized by the scalar levels
@@ -305,8 +316,10 @@ int32_t scpb_cone_setup(scpb_handle h, int32_t n, int32_t p, int32_t m, const in
     P.fwp_lvl = upload_ints(c, S.fwp_lvl); P.bwp_lvl = upload_ints(c, S.bwp_lvl);
     P.fwp_R = upload_ints(c, S.fwp_R); P.bwp_R = upload_ints(c, S.bwp_R);
     P.Lr_pc = (const int2 *)upload_ints(c, S.Lr_pc); P.ft_op = (const int2 *)upload_ints(c, S.ft_op);
-    P.fc_item = (const int4 *)upload_ints(c, S.fc_item); P.fwc_item = (const int4 *)upload_ints(c, S.fwc_item);
+    P.fwc_item = (const int4 *)upload_ints(c, S.fwc_item);
     P.bwc_item = (const int4 *)upload_ints(c, S.bwc_item);
+    P.fb_cmb = (const int4 *)upload_ints(c, S.fb_cmb);
+    P.npf = S.fslots; P.nps = S.sslots;
     // hybrid program: SCPB_HYBRID=<cut> (supernodal level at which the in-place panels take over; 0 = off)
     {
         const char *e = getenv("SCPB_HYBRID");
@@ -321,8 +334,10 @@ int32_t scpb_cone_setup(scpb_handle h, int32_t n, int32_t p, int32_t m, const in
             H.fwp_item = (const int4 *)upload_ints(c, S.hy_fwp_item); H.bwp_item = (const int4 *)upload_ints(c, S.hy_bwp_item);
             H.fwp_lvl = upload_ints(c, S.hy_fwp_lvl); H.bwp_lvl = upload_ints(c, S.hy_bwp_lvl);
             H.fwp_R = upload_ints(c, S.hy_fwp_R); H.bwp_R = upload_ints(c, S.hy_bwp_R);
-            H.fc_item = (const int4 *)upload_ints(c, S.hy_fc_item); H.fwc_item = (const int4 *)upload_ints(c, S.hy_fwc_item);
+            H.fwc_item = (const int4 *)upload_ints(c, S.hy_fwc_item);
             H.bwc_item = (const int4 *)upload_ints(c, S.hy_bwc_item);
+            H.fb_cmb = (const int4 *)upload_ints(c, S.hy_fb_cmb);
+            H.npf = S.hy_fslots; H.nps = S.hy_sslots;
             H.hy.desc = (const int4 *)upload_ints(c, S.hy_desc); H.hy.tl_ptr = upload_ints(c, S.hy_tl_ptr);
             H.hy.upd_dst = upload_ints(c, S.hy_upd_dst); H.hy.rows = P.sn.rows; H.hy.ntl = S.hy_ntl;
             c->hy_ok = true;

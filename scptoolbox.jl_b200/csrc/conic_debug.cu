@@ -5,21 +5,27 @@
 #include "../../include/scpb.h"
 #include "conic_symbolic.h"
 
-// An item's partial sum, applied the way k_ipm_solve applies it: straight to the target, or, for an item of a split
-// target (.w = 1 + slot, conic_symbolic.h: number_pieces), into its slot, the last item of the target subtracting the
-// slots in slot order.  add() fails when the slot does not belong to the item's target; level_done() fails when a
-// target of the level did not receive all the items its slot range promises.
+// Partial sums of split targets, applied the way k_ipm_solve applies them (conic_symbolic.h: number_pieces,
+// combine_in_phase_b); slots are numbered from 0 in every level.
+// Substitutions, add(): an item of a split target (.w = 1 + index into info) stores its sum in its slot, and the last
+// item of the target subtracts the target's slots in slot order.  add() fails when the info entry belongs to another
+// target or its slot lies outside the target's range; level_done() fails when a target of the level did not receive
+// all the items its slot range promises.
+// Factorisation, store() / take(): phase A stores an item's sum in slot .w - 1, phase B subtracts the slot ranges of
+// fb_cmb.  take() fails when a range holds a slot that this level's phase A did not store for that target;
+// level_done() fails when a stored slot was not taken exactly once as the entry of a phase-B item.
 struct SplitSums {
     std::vector<double> part;
-    std::vector<int> cnt;
-    explicit SplitSums(int npart) : part((size_t)npart + 1, 0.0), cnt((size_t)npart + 1, 0) {}
+    std::vector<int> cnt, tgt, taken;
+    explicit SplitSums(int nslot) : part((size_t)nslot, 0.0), cnt((size_t)nslot, 0), tgt((size_t)nslot, -1), taken((size_t)nslot, 0) {}
     bool add(const int *it, const std::vector<int> &info, double p, double *y)
     {
         if (!it[3]) { y[it[0]] -= p; return true; }
-        const int sl = it[3] - 1;
-        if (sl < 0 || 4 * (size_t)sl + 3 >= info.size()) return false;
-        const int *e = &info[4 * (size_t)sl];
-        if (e[0] != it[0] || sl < e[1] || sl >= e[2]) return false;
+        const size_t q = (size_t)it[3] - 1;
+        if (it[3] < 1 || 4 * q + 3 >= info.size()) return false;
+        const int *e = &info[4 * q];
+        const int sl = e[3];
+        if (e[0] != it[0] || e[1] < 0 || e[2] > (int)part.size() || sl < e[1] || sl >= e[2]) return false;
         part[sl] = p;
         if (++cnt[e[1]] == e[2] - e[1]) {
             double acc = y[e[0]];
@@ -29,12 +35,47 @@ struct SplitSums {
         }
         return true;
     }
-    bool level_done() const
+    bool store(const int *it, double p, double *y)
     {
-        for (int c : cnt) if (c) return false;
+        if (!it[3]) { y[it[0]] -= p; return true; }
+        const int sl = it[3] - 1;
+        if (sl < 0 || sl >= (int)part.size() || tgt[sl] >= 0) return false;
+        part[sl] = p; tgt[sl] = it[0];
         return true;
     }
+    bool take(int t, int s0, int s1, double &acc, bool entry)
+    {
+        for (int k = s0; k < s1; k++) {
+            if (k < 0 || k >= (int)part.size() || tgt[k] != t) return false;
+            acc -= part[k];
+            taken[k] += entry;
+        }
+        return true;
+    }
+    bool level_done()
+    {
+        bool ok = true;
+        for (size_t k = 0; k < cnt.size(); k++) {
+            if (cnt[k] || (tgt[k] >= 0 && taken[k] != 1)) ok = false;
+            tgt[k] = -1; taken[k] = 0;
+        }
+        return ok;
+    }
 };
+
+// Phase B's operands of a factorisation item: its entry and the pivot of its column, each minus the slots of its split
+// target.  The entry is written back, because later levels read it; the pivot is not, because the other items of the
+// column read it in the same phase (the diagonal item keeps the combined pivot in e).
+static bool phase_b_operands(SplitSums &split, const int *it, const int *cm, int nnzL, std::vector<double> &Y, double &e, double &d)
+{
+    e = Y[it[0]];
+    if (!split.take(it[0], cm[0], cm[1], e, true)) return false;
+    if (it[3] & 2) { d = e; return true; }
+    d = Y[(size_t)nnzL + it[1]];
+    if (!split.take(nnzL + it[1], cm[2], cm[3], d, false)) return false;
+    Y[it[0]] = e;
+    return true;
+}
 
 extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const int32_t *A_rp, const int32_t *A_ci,
                                         const int32_t *G_rp, const int32_t *G_ci, int32_t l, int32_t nsoc,
@@ -63,18 +104,19 @@ extern "C" int32_t scpb_debug_kkt_solve(int32_t n, int32_t p, int32_t m, const i
             if (it[2] - it[1] > R * CONIC_FACTOR_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Y[S.ft_op[2 * (size_t)k]] * Ls[S.Lr_pos[S.ft_op[2 * (size_t)k + 1]]];
-            if (!split.add(it, S.fc_item, part, Y.data())) return SCPB_ERR_ARG;
+            if (!split.store(it, part, Y.data())) return SCPB_ERR_ARG;
             nsplit += it[3] != 0;
         }
-        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.fb_lvl[lv]; w < S.fb_lvl[lv + 1]; w++) {   // every item regularises its own copy of the pivot
             const int *it = &S.fb_item[4 * (size_t)w];
+            double e, d;
+            if (!phase_b_operands(split, it, &S.fb_cmb[4 * (size_t)w], S.nnzL, Y, e, d)) return SCPB_ERR_ARG;
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;
-            double d = Y[S.nnzL + it[1]];
             if (!(sgn * d > delta_dyn)) d = sgn * delta_dyn;
             if (it[3] & 2) invD[it[1]] = 1.0 / d;
-            else Ls[it[0]] = Y[it[0]] * (1.0 / d);
+            else Ls[it[0]] = e * (1.0 / d);
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int i = 0; i < nk; i++) v[S.iperm[i]] = rhs[i];
     // kkt_ldl_solve_smem: the balanced (split-item) substitution programs, level by level; within a level every
@@ -222,17 +264,19 @@ extern "C" int32_t scpb_debug_kkt_solve_hy(int32_t n, int32_t p, int32_t m, cons
             if (it[2] - it[1] > R * CONIC_FACTOR_PF) return SCPB_ERR_ARG;
             double part = 0.0;
             for (int k = it[1]; k < it[2]; k++) part += Y[S.hy_ft_op[2 * (size_t)k]] * Ls[S.Lr_pos[S.hy_ft_op[2 * (size_t)k + 1]]];
-            if (!split.add(it, S.hy_fc_item, part, Y.data())) return SCPB_ERR_ARG;
+            if (!split.store(it, part, Y.data())) return SCPB_ERR_ARG;
         }
-        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.hy_fb_lvl[lv]; w < S.hy_fb_lvl[lv + 1]; w++) {
             const int *it = &S.hy_fb_item[4 * (size_t)w];
+            double e, d;
+            if (!phase_b_operands(split, it, &S.hy_fb_cmb[4 * (size_t)w], S.nnzL, Y, e, d)) return SCPB_ERR_ARG;
+            if (it[3] & 4) continue;   // combine-only item of the bridge level: the top panels finish the target
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;
-            double d = Y[S.nnzL + it[1]];
             if (!(sgn * d > delta_dyn)) d = sgn * delta_dyn;
             if (it[3] & 2) invD[it[1]] = 1.0 / d;
-            else Ls[it[0]] = Y[it[0]] * (1.0 / d);
+            else Ls[it[0]] = e * (1.0 / d);
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     // panel entry (r, c) of a top supernode, r >= c, as a target id / L position
     auto ppos = [&](const int *d, int r, int c) { return r == c ? S.nnzL + d[0] + c : d[3] + c * (d[2] - 1) - (c * (c - 1)) / 2 + (r - c - 1); };
@@ -382,20 +426,21 @@ extern "C" int32_t scpb_debug_kkt_factor(void *h, const double *Av, const double
             const int *it = &S.fa_item[4 * (size_t)w];
             double part = 0.0;
             for (int q = it[1]; q < it[2]; q++) part += Y[S.ft_op[2 * (size_t)q]] * Ls[S.Lr_pos[S.ft_op[2 * (size_t)q + 1]]];
-            if (!split.add(it, S.fc_item, part, Y.data())) return SCPB_ERR_ARG;
+            if (!split.store(it, part, Y.data())) return SCPB_ERR_ARG;
         }
-        if (!split.level_done()) return SCPB_ERR_ARG;
         for (int w = S.fb_lvl[lv]; w < S.fb_lvl[lv + 1]; w++) {
             const int *it = &S.fb_item[4 * (size_t)w];
+            double e, d;
+            if (!phase_b_operands(split, it, &S.fb_cmb[4 * (size_t)w], S.nnzL, Y, e, d)) return SCPB_ERR_ARG;
             const double sgn = (it[3] & 1) ? 1.0 : -1.0;
-            double d = Y[S.nnzL + it[1]];
             if (!(sgn * d > tau)) {
                 if (it[3] & 2) { nreg++; if (!(std::abs(d) <= bad_abs)) nbad++; }
                 d = sgn * rho;
             }
             if (it[3] & 2) { invD[it[1]] = 1.0 / d; dmin = std::min(dmin, std::abs(d)); }
-            else { Ls[it[0]] = Y[it[0]] * (1.0 / d); lmax = std::max(lmax, std::abs(Ls[it[0]])); }
+            else { Ls[it[0]] = e * (1.0 / d); lmax = std::max(lmax, std::abs(Ls[it[0]])); }
         }
+        if (!split.level_done()) return SCPB_ERR_ARG;
     }
     for (int q = 0; q < S.nnzL; q++) k->Lrow[q] = Ls[S.Lr_pos[q]];
     if (!(lmax < 1e300)) nbad++;

@@ -38,8 +38,10 @@ struct IpmProgram {  // device copies of ConeSymbolic index arrays
     const int *fa_lvl, *fa_R, *fb_lvl;
     const int *fwp_lvl, *bwp_lvl, *fwp_R, *bwp_R;
     const int2 *Lr_pc, *ft_op;
-    const int4 *fc_item, *fwc_item, *bwc_item;   // per partial-sum slot: {target, first slot, end slot, 0} (conic_symbolic.h)
-    int npart;                                   // partial-sum slots per seed
+    const int4 *fwc_item, *bwc_item;             // per split item: {target, first slot, end slot, slot} (conic_symbolic.h)
+    const int4 *fb_cmb;                          // per phase-B item: slot ranges of its entry and of its pivot
+    int npart;                                   // partial-sum slots per seed in global memory (all programs)
+    int npf, nps;                                // the most slots of one level: factorisation, substitutions
 };
 
 struct IpmOpts {
@@ -74,9 +76,10 @@ struct IpmData {  // group-blocked device arrays, all for B seeds
     // work
     double *rx, *ry, *rz, *lam, *wm, *socw, *soceta;
     double *dx, *dy, *dz, *ds, *dsa, *dza, *tm, *gm, *r1, *r2, *e1, *e2, *rhs, *Y, *Ls, *Lrow, *invD;
-    double *part;   // partial sums of split targets (IpmProgram.npart slots per seed)
-    double *pcnt;   // storage of the split targets' finished-item counters (unsigned, zero between uses)
+    double *part;   // partial sums of split targets (IpmProgram.npart slots per seed), unless psmem
+    double *pcnt;   // storage of the split targets' finished-item counters (unsigned, zero between uses), unless psmem
     int vsmem;   // 1: the substitution vector of kkt_ldl_solve lives in shared memory (nk*G doubles fit)
+    int psmem;   // 1: the partial sums and counters of a level live in shared memory too (vsmem, and they fit)
     // per-seed outputs
     double *pobj, *dobj, *res;   // res: [3][B] pres, dres, gap
     int *status, *iters;
@@ -120,8 +123,8 @@ struct Ctx {
     double rho_min, bad_abs;
     double *vs;                         // shared-memory substitution vector (nullptr: use global memory)
     double *Lrow;                       // row-ordered copy of the scaled factor (forward substitution)
-    double *part;                       // partial sums of the split targets of a level
-    unsigned *pcnt;                     // ... and their finished-item counters
+    double *fpart, *spart;              // partial sums of the split targets of a level: factorisation, substitutions
+    unsigned *pcnt;                     // ... and the substitutions' finished-item counters
     double reftol;                      // iterative refinement stops once |residual|_inf <= reftol*(1+|rhs|_inf) ...
     const double *s_mu;                 // ... reftol while the seed's complementarity gap/deg is above mu_tight, 1e-13 below it
     double mu_tight;                    //     (shared: per-seed mu of the current iterate)
@@ -253,36 +256,44 @@ __device__ __forceinline__ void kkt_assemble(const IpmProgram &P, const Ctx &c, 
 
 // ---- numeric LDL' : balanced, level-scheduled gather program (conic_symbolic.h, "balanced factorisation program") ----
 // Phase A of a level: an item subtracts at most R*IPM_FPF products Y[a]*Ls[b] from one target; a lane owns at most
-// IPM_FPF of them, so all its op indices and then all its gathers are in flight together.  Targets whose op list was
-// split store their partial sums in slots that the last of them subtracts in slot order (ipm_split_done; every read of Y
-// goes to L2, ld.cg).  Phase B finishes
-// the level's columns: each item regularises its own copy of the pivot, the diagonal item stores 1/d, the others
-// scale their entry and store it twice (column order for the backward sweep, row order for the forward sweep).
+// IPM_FPF of them, so all its op indices and then all its gathers are in flight together.  An item of a target whose op
+// list was split only stores its partial sum in its slot (numbered per level, conic_symbolic.h: combine_in_phase_b);
+// the slots of a level live in shared memory (the window of the substitution vector, which is free while the
+// factorisation runs) or, when they do not fit, in global memory.  Every read of Y goes to L2 (ld.cg).  Phase B
+// finishes the level's columns behind the level's barrier: each item subtracts the slots of its entry and of its
+// column's pivot in slot order as it reads them (the same bits in every item of the column, and the same bits as
+// summing them in any other place in that order), regularises its own copy of the pivot; the diagonal item stores 1/d,
+// the others write the combined entry back to Y for the later levels, scale it and store it twice (column order for the
+// backward sweep, row order for the forward sweep).  Combine-only items (flag 4, the hybrid program's bridge level) just
+// write their combined target back.  No fence, no atomic: the level's barrier orders the slots.
 // The program data of the next phase (item descriptors, op indices) is requested one phase early.
 // Separate (noinline) function with by-value arguments: see solve_sweep.
 #define IPM_FPF CONIC_FACTOR_PF
-// An item of a split target stores its partial sum in its slot and counts itself in; the last item of the target to
-// finish subtracts all slots from the target in slot order (and resets the counter), so the sum does not depend on the
-// order in which the items ran.  Returns true in the thread that has to do that.
-__device__ __forceinline__ bool ipm_split_done(double *part, unsigned *cnt, int4 e, int sl, double v, int G, int sg)
+// Substitutions: an item of a split target stores its partial sum in its slot and counts itself in; the last item of
+// the target to finish subtracts all slots from the target in slot order (and resets the counter), so the sum does not
+// depend on the order in which the items ran.  Returns true in the thread that has to do that.  Slots and counters are
+// the level's, in shared memory (or global memory when they do not fit): the block-scope fence and atomic are all the
+// ordering the CTA-local hand-over needs.
+__device__ __forceinline__ bool ipm_split_done(double *part, unsigned *cnt, int4 e, double v, int G, int sg)
 {
-    part[(size_t)sl * G + sg] = v;
+    part[e.w * G + sg] = v;
     __threadfence_block();
-    const bool last = atomicAdd(&cnt[(size_t)e.y * G + sg], 1u) == (unsigned)(e.z - e.y - 1);
-    if (last) { __threadfence_block(); cnt[(size_t)e.y * G + sg] = 0u; }
+    const bool last = atomicAdd(&cnt[e.y * G + sg], 1u) == (unsigned)(e.z - e.y - 1);
+    if (last) { __threadfence_block(); cnt[e.y * G + sg] = 0u; }
     return last;
 }
-__device__ __forceinline__ double ipm_split_sum(const double *part, int4 e, double acc, int G, int sg)
+// acc minus the slots [k0, k1) in slot order
+__device__ __forceinline__ double ipm_split_sum(const double *part, int k0, int k1, double acc, int G, int sg)
 {
-    for (int k = e.y; k < e.z; k++) acc -= __ldcg(&part[(size_t)k * G + sg]);
+    for (int k = k0; k < k1; k++) acc -= part[k * G + sg];
     return acc;
 }
 struct FactorArgs {
     const int4 *fa_item, *fb_item;
     const int2 *ft_op;
-    const int4 *fc_item;            // partial-sum slots of the split targets
-    double *Y, *Ls, *Lrow, *invD, *part;   // group-blocked, already offset to this CTA's group
-    unsigned *pcnt;
+    const int4 *fb_cmb;             // per phase-B item: slot ranges of its entry and of its pivot
+    double *Y, *Ls, *Lrow, *invD;   // group-blocked, already offset to this CTA's group
+    double *part;                   // partial sums of the level's split targets (shared or global memory)
     int o_fal, o_faR, o_fbl;        // offsets (ints) into the dynamic shared memory window
     int nl, nnzLd, G, sg, slot, nslots;
     long long *lprof;
@@ -334,8 +345,8 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
         const int R = faR[lv], nisl = nslots >> (31 - __clz(R));
         const int nA = fal[lv + 1] - fal[lv];
         const int b0 = fbl[lv], b1 = fbl[lv + 1];
-        int4 sc = make_int4(-1, 0, 0, 0);                    // first phase-B item of this lane, requested early
-        if (b0 + slot < b1) sc = a.fb_item[b0 + slot];
+        int4 sc = make_int4(-1, 0, 0, 0), sr = make_int4(0, 0, 0, 0);   // first phase-B item of this lane and its slot
+        if (b0 + slot < b1) { sc = a.fb_item[b0 + slot]; sr = a.fb_cmb[b0 + slot]; }   // ranges, requested early
         for (int off = 0; off < nA; off += nisl) {
             double ya_[IPM_FPF], la_[IPM_FPF];
 #pragma unroll
@@ -352,14 +363,8 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
             for (int j = 0; j < IPM_FPF; j++) part_ = fma(ya_[j], la_[j], part_);
             for (int o_ = G; o_ < G * R; o_ <<= 1) part_ += __shfl_xor_sync(0xffffffffu, part_, o_);
             if (t_tgt >= 0 && (slot & (R - 1)) == 0) {
-                if (t_tgt >> 30) {
-                    const int sl_ = t_tgt & 0x3fffffff;
-                    const int4 e_ = a.fc_item[sl_];
-                    if (ipm_split_done(a.part, a.pcnt, e_, sl_, part_, G, sg)) {
-                        double *p_ = &a.Y[(size_t)e_.x * G + sg];
-                        *p_ = ipm_split_sum(a.part, e_, __ldcg(p_), G, sg);
-                    }
-                } else { double *p_ = &a.Y[(size_t)t_tgt * G + sg]; *p_ = __ldcg(p_) - part_; }
+                if (t_tgt >> 30) a.part[(t_tgt & 0x3fffffff) * G + sg] = part_;   // phase B combines it
+                else { double *p_ = &a.Y[(size_t)t_tgt * G + sg]; *p_ = __ldcg(p_) - part_; }
             }
             t_tgt = n_tgt;
 #pragma unroll
@@ -372,10 +377,17 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
         for (int w = b0 + slot; w < b1; w += nslots) {
             const double sgn = (sc.w & 1) ? 1.0 : -1.0;
             const bool isd = (sc.w & 2) != 0;
-            const double e = __ldcg(&a.Y[(size_t)sc.x * G + sg]);
-            double d = isd ? e : __ldcg(&a.Y[(size_t)(a.nnzLd + sc.y) * G + sg]);
-            const int4 cur = sc;
-            if (w + nslots < b1) sc = a.fb_item[w + nslots];
+            double e = __ldcg(&a.Y[(size_t)sc.x * G + sg]);
+            double d = isd ? 0.0 : __ldcg(&a.Y[(size_t)(a.nnzLd + sc.y) * G + sg]);
+            const int4 cur = sc, cr = sr;
+            if (w + nslots < b1) { sc = a.fb_item[w + nslots]; sr = a.fb_cmb[w + nslots]; }
+            e = ipm_split_sum(a.part, cr.x, cr.y, e, G, sg);
+            if (isd) d = e;
+            else {
+                d = ipm_split_sum(a.part, cr.z, cr.w, d, G, sg);
+                if (cr.y > cr.x) a.Y[(size_t)cur.x * G + sg] = e;   // a later level reads it as an operand
+                if (cur.w & 4) continue;                            // combine-only item
+            }
             const double dl_ = ipm_s_delta[sg];
             if (!(sgn * d > 0.5 * dl_)) {   // dynamic regularisation keeps the expected inertia
                 if (isd && !(fabs(d) <= ipm_s_reg[1])) ipm_s_bad[sg] = 1;   // not a small pivot: cancellation destroyed it
@@ -579,8 +591,8 @@ __device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *
 {
     if constexpr (SN == 1) { kkt_factor_sn(c.s_sn, c.tid); return; }
     FactorArgs a;
-    a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fc_item = P.fc_item;
-    a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.part; a.pcnt = c.pcnt;
+    a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fb_cmb = P.fb_cmb;
+    a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.fpart;
     a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
     a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = c.G; a.sg = c.sg; a.slot = c.slot; a.nslots = c.nslots;
     a.lprof = c.lprof;
@@ -593,7 +605,9 @@ __device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *
 // R*IPM_PF entries (conic_symbolic.h, "balanced substitution programs"), so a lane never owns more than IPM_PF
 // entries of an item: right after a level's items are consumed the lane issues ALL global loads of the next level
 // (indices + values, through an item descriptor fetched one level earlier) and only then waits at the barrier.
-// Items of a split row store their partial sums in slots that the last of them subtracts in slot order.
+// Items of a split row store their partial sums in slots that the last of them subtracts in slot order
+// (ipm_split_done); the slots and counters of a level live in shared memory after the vector (global memory when they
+// do not fit).
 // The sweep is a separate (noinline) function with by-value arguments and shared-window pointers: its register
 // allocation is independent of the 60+ live pointers of the solver body, so the prefetch registers are not spilled
 // (a spilled prefetch is a synchronous load).
@@ -602,8 +616,8 @@ struct SweepArgs {
     const int4 *items;      // balanced items {node, start, end, split}
     const int *idxarr;      // entry -> vector index (column of the row entry / row of the column entry)
     const double *vals;     // group-blocked L values in the same entry order
-    const int4 *cmb;        // partial-sum slots of the split rows / columns
-    double *part;           // group-blocked partial-sum slots and their counters
+    const int4 *cmb;        // split items: {row / column, first slot, end slot, slot}
+    double *part;           // partial sums of the level's split rows / columns, and their counters
     unsigned *pcnt;
     int o_lvl, o_R, o_vs;   // offsets (ints) into the dynamic shared memory window
     int nl, lv0, G, sg, slot, nslots;
@@ -652,10 +666,9 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
         for (int o_ = G; o_ < G * (R); o_ <<= 1) part_ += __shfl_xor_sync(0xffffffffu, part_, o_); \
         if (q_node >= 0 && (slot & ((R) - 1)) == 0) {                                     \
             if (q_node >> 30) {                                                           \
-                const int sl_ = q_node & 0x3fffffff;                                      \
-                const int4 e_ = a.cmb[sl_];                                               \
-                if (ipm_split_done(a.part, a.pcnt, e_, sl_, part_, G, sg))                \
-                    vs[e_.x * G + sg] = ipm_split_sum(a.part, e_, vs[e_.x * G + sg], G, sg); \
+                const int4 e_ = a.cmb[q_node & 0x3fffffff];                               \
+                if (ipm_split_done(a.part, a.pcnt, e_, part_, G, sg))                     \
+                    vs[e_.x * G + sg] = ipm_split_sum(a.part, e_.y, e_.z, vs[e_.x * G + sg], G, sg); \
             } else vs[q_node * G + sg] -= part_;                                          \
         }                                                                                 \
     }
@@ -696,7 +709,7 @@ __device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c, 
     const long long t0_ = clock64();
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
     SweepArgs a;
-    a.nl = P.nlevels; a.G = G; a.sg = sg; a.slot = c.slot; a.nslots = c.nslots; a.o_vs = c.o_vs; a.part = c.part; a.pcnt = c.pcnt;
+    a.nl = P.nlevels; a.G = G; a.sg = sg; a.slot = c.slot; a.nslots = c.nslots; a.o_vs = c.o_vs; a.part = c.spart; a.pcnt = c.pcnt;
     // forward: level 0 rows are empty (leaves have no dependencies); the barrier inside the sweep publishes vs
     a.items = P.fwp_item; a.idxarr = P.Lr_col; a.vals = c.Lrow; a.o_lvl = c.o_fwl; a.o_R = c.o_fwR; a.lv0 = 1;
     a.cmb = P.fwc_item;
@@ -1174,8 +1187,16 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         s_snargs = a;
     }
     c.Lrow = GP(D.Lrow, P.nnzL + 1);
-    c.part = GP(D.part, P.npart + 1);
-    c.pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
+    if (D.psmem) {   // dynamic window: level pointers | vector, or the factorisation's slots | substitution slots | counters
+        const int vw = 2 * (P.nk > P.npf ? P.nk : P.npf) * G;
+        c.fpart = (double *)(s_lv + c.o_vs);
+        c.spart = (double *)(s_lv + c.o_vs + vw);
+        c.pcnt = (unsigned *)(s_lv + c.o_vs + vw + 2 * P.nps * G);
+        for (int i = c.tid; i < P.nps * G; i += NT) c.pcnt[i] = 0u;   // the barrier below publishes it
+    } else {
+        c.fpart = c.spart = GP(D.part, P.npart + 1);
+        c.pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
+    }
 #undef GP
 
     long long pt[8] = {0, 0, 0, 0, 0, 0, 0, 0};

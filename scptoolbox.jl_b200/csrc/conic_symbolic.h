@@ -87,8 +87,12 @@ struct ConeSymbolic {
     // bit1 = the item is the diagonal itself (regularise, write 1/d), otherwise scale the entry by 1/d.
     std::vector<int> fa_item, fa_lvl, fa_R;
     std::vector<int> fb_item, fb_lvl;
-    // partial-sum slots of the split targets: int4 per slot {target, first slot, end slot of the target, 0} (number_pieces)
+    // split targets (number_pieces): int4 per split item {target, first slot, end slot of the target, slot}, slots
+    // numbered from 0 in every level.  The substitution items point into these (.w = 1 + index); the factorisation's
+    // phase-A items hold their slot itself (.w = 1 + slot), and phase B combines the split targets through fb_cmb.
     std::vector<int> fc_item, fwc_item, bwc_item;
+    std::vector<int> fb_cmb;          // int4 per phase-B item: {entry first slot, entry end slot, pivot first slot, pivot end slot}
+    int fslots = 0, sslots = 0;       // the most slots of one level: factorisation, substitutions (forward or backward)
     int npart = 0;                    // partial-sum slots per seed: the most any of the programs (hybrid included) uses
     // ---- supernodal program (executed by the kernels of conic_sn.cuh; CPU interpreter scpb_debug_kkt_solve_sn,
     // tests/test_conic_symbolic.py) ----
@@ -116,7 +120,8 @@ struct ConeSymbolic {
     int hy_cut = 0, hy_nlevels = 0, hy_ntl = 0;
     std::vector<int> hy_fa_item, hy_fa_lvl, hy_fa_R, hy_fb_item, hy_fb_lvl, hy_ft_op;
     std::vector<int> hy_fwp_item, hy_fwp_lvl, hy_fwp_R, hy_bwp_item, hy_bwp_lvl, hy_bwp_R;
-    std::vector<int> hy_fc_item, hy_fwc_item, hy_bwc_item;
+    std::vector<int> hy_fc_item, hy_fwc_item, hy_bwc_item, hy_fb_cmb;
+    int hy_fslots = 0, hy_sslots = 0;
     std::vector<int> hy_tl_ptr;     // hy_ntl + 1 -> index into the descriptor list
     std::vector<int> hy_desc;       // 8 ints per top supernode in top-level order: {first column, width, rows, L_cp[first]},
                                     // {offset into sn_rows, offset into hy_upd_dst, pivot signs (bit c: column c expects +), 0}
@@ -131,30 +136,91 @@ struct ConeSymbolic {
 
 namespace conic_detail {
 
-// Items whose target is split over several items (.w != 0 on input) get a partial-sum slot each: .w = 1 + slot.  The
-// kernels store such an item's partial sum in its slot and count the finished items of the target; the last one
-// subtracts the target's slots from it in slot order, so the result does not depend on the order in which the items
-// ran.  info[slot] = {target, first slot, end slot of the target, 0}; the first slot also numbers the target's counter.
-inline void number_pieces(std::vector<int> &item, const std::vector<int> &lvl, std::vector<int> &info, int &npart)
+// Items whose target is split over several items (.w != 0 on input) get a partial-sum slot each.  Slots are numbered
+// from 0 in every level, so that the slots of one level fit in shared memory; a target's slots are consecutive, in
+// item order.  .w = 1 + index of the split item in info; info[index] = {target, first slot, end slot of the target,
+// slot}.  The substitution kernels store an item's partial sum in its slot and count the finished items of the target
+// (the counter is numbered by the first slot); the last one subtracts the target's slots from it in slot order, so the
+// result does not depend on the order in which the items ran.  nslot: the most slots of one level.
+inline void number_pieces(std::vector<int> &item, const std::vector<int> &lvl, std::vector<int> &info, int &nslot)
 {
     const int nl = (int)lvl.size() - 1;
     info.clear();
-    int slot = 0;
+    nslot = 0;
     for (int lv = 0; lv < nl; lv++) {
         std::vector<std::pair<int, int>> sp;   // (target, item) of the split items of the level
         for (int w = lvl[lv]; w < lvl[lv + 1]; w++)
             if (item[4 * (size_t)w + 3]) sp.push_back({item[4 * (size_t)w], w});
         std::stable_sort(sp.begin(), sp.end(), [](const std::pair<int, int> &x, const std::pair<int, int> &y) { return x.first < y.first; });
+        int slot = 0;
         for (size_t i = 0; i < sp.size();) {
-            const int s0 = slot;
             size_t j = i;
-            for (; j < sp.size() && sp[j].first == sp[i].first; j++) item[4 * (size_t)sp[j].second + 3] = 1 + slot++;
-            for (int k = s0; k < slot; k++) { info.push_back(sp[i].first); info.push_back(s0); info.push_back(slot); info.push_back(0); }
-            i = j;
+            while (j < sp.size() && sp[j].first == sp[i].first) j++;
+            const int s0 = slot, s1 = slot + (int)(j - i);
+            for (; i < j; i++) {
+                item[4 * (size_t)sp[i].second + 3] = 1 + (int)(info.size() / 4);
+                info.push_back(sp[i].first); info.push_back(s0); info.push_back(s1); info.push_back(slot++);
+            }
         }
+        nslot = std::max(nslot, slot);
     }
     if (info.empty()) info.assign(4, 0);
-    npart = std::max(npart, slot);
+}
+
+// The factorisation combines its split targets without counters: phase A only stores the partial sums in their slots
+// (.w is rewritten to 1 + slot), and phase B, which follows the level's barrier and reads every target of its level --
+// the entry it scales and the pivot of its column -- subtracts their slots in slot order as it reads them.  cmb gets an
+// int4 per phase-B item {entry first slot, entry end slot, pivot first slot, pivot end slot} (empty ranges: target not
+// split).  Every split target must be the entry of exactly one phase-B item of its level, which writes the combined
+// value back to Y for the later levels.  A split target that no phase-B item of its level finishes (the bridge level
+// of the hybrid program, whose targets the top panels finish) gets a combine-only phase-B item {target, 0, 0, 4} when
+// `extra` is set; otherwise the build fails.  Without `extra` every phase-A target must be an entry of phase B.
+inline bool combine_in_phase_b(std::vector<int> &fa, const std::vector<int> &fal, const std::vector<int> &info,
+                               std::vector<int> &fb, std::vector<int> &fbl, std::vector<int> &cmb, int ntgt, int nnzL,
+                               bool extra)
+{
+    const int nl = (int)fal.size() - 1;
+    std::vector<int> nfb, stamp(ntgt, -1), r0(ntgt, 0), r1(ntgt, 0), used(ntgt, 0), entry(ntgt, -1);
+    cmb.clear();
+    for (int lv = 0; lv < nl; lv++) {
+        for (int w = fal[lv]; w < fal[lv + 1]; w++) {
+            int *it = &fa[4 * (size_t)w];
+            if (it[0] < 0 || it[0] >= ntgt) return false;
+            stamp[it[0]] = lv; used[it[0]] = 0;
+            if (!it[3]) { r0[it[0]] = r1[it[0]] = 0; continue; }
+            const int *e = &info[4 * (size_t)(it[3] - 1)];
+            if (e[0] != it[0]) return false;
+            r0[it[0]] = e[1]; r1[it[0]] = e[2];
+            it[3] = 1 + e[3];
+        }
+        for (int w = fbl[lv]; w < fbl[lv + 1]; w++) {
+            const int *it = &fb[4 * (size_t)w];
+            const int t = it[0], pv = nnzL + it[1];
+            const bool te = stamp[t] == lv, tp = stamp[pv] == lv;
+            for (int q = 0; q < 4; q++) nfb.push_back(it[q]);
+            cmb.push_back(te ? r0[t] : 0); cmb.push_back(te ? r1[t] : 0);
+            cmb.push_back(tp ? r0[pv] : 0); cmb.push_back(tp ? r1[pv] : 0);
+            if (te) { used[t]++; entry[t] = lv; }
+        }
+        for (int w = fal[lv]; w < fal[lv + 1]; w++) {
+            const int t = fa[4 * (size_t)w];
+            if (entry[t] == lv) {
+                if (used[t] != 1) return false;   // two phase-B items would write the same target back
+                continue;
+            }
+            if (!extra) return false;             // a target of phase A that phase B of its level does not finish
+            if (r1[t] > r0[t]) {
+                nfb.push_back(t); nfb.push_back(0); nfb.push_back(0); nfb.push_back(4);
+                cmb.push_back(r0[t]); cmb.push_back(r1[t]); cmb.push_back(0); cmb.push_back(0);
+                used[t] = 1; entry[t] = lv;
+            }
+        }
+        fbl[lv + 1] = (int)(nfb.size() / 4);
+    }
+    if (nfb.empty()) nfb.assign(4, 0);
+    if (cmb.empty()) cmb.assign(4, 0);
+    fb.swap(nfb);
+    return true;
 }
 
 inline void transpose_pattern(int nrow, int ncol, const std::vector<int> &rp, const std::vector<int> &ci,
@@ -471,7 +537,12 @@ inline bool cone_symbolic_build(ConeSymbolic &S, int n, int p, int m, const int 
             S.fb_lvl[lv + 1] = (int)(S.fb_item.size() / 4);
         }
         if (S.fa_item.empty()) S.fa_item.assign(4, 0);
-        conic_detail::number_pieces(S.fa_item, S.fa_lvl, S.fc_item, S.npart);
+        conic_detail::number_pieces(S.fa_item, S.fa_lvl, S.fc_item, S.fslots);
+        if (!conic_detail::combine_in_phase_b(S.fa_item, S.fa_lvl, S.fc_item, S.fb_item, S.fb_lvl, S.fb_cmb, S.nnzL + nk,
+                                              S.nnzL, false)) {
+            S.err = "internal: a phase-A target of the factorisation is not finished by one phase-B item of its level";
+            return false;
+        }
     }
     // ---- supernodal program ----
     {
@@ -613,9 +684,12 @@ inline bool cone_symbolic_build(ConeSymbolic &S, int n, int p, int m, const int 
         };
         build(S.Lr_rp, S.fwp_item, S.fwp_lvl, S.fwp_R);
         build(S.L_cp, S.bwp_item, S.bwp_lvl, S.bwp_R);
-        conic_detail::number_pieces(S.fwp_item, S.fwp_lvl, S.fwc_item, S.npart);
-        conic_detail::number_pieces(S.bwp_item, S.bwp_lvl, S.bwc_item, S.npart);
+        int fw_ = 0, bw_ = 0;
+        conic_detail::number_pieces(S.fwp_item, S.fwp_lvl, S.fwc_item, fw_);
+        conic_detail::number_pieces(S.bwp_item, S.bwp_lvl, S.bwc_item, bw_);
+        S.sslots = std::max(fw_, bw_);
     }
+    S.npart = std::max(S.fslots, S.sslots);
     return true;
 }
 
@@ -700,8 +774,12 @@ inline bool cone_symbolic_build_hybrid(ConeSymbolic &S, int cut)
             S.hy_fb_lvl[lv + 1] = (int)(S.hy_fb_item.size() / 4);
         }
         if (S.hy_fa_item.empty()) S.hy_fa_item.assign(4, 0);
-        if (S.hy_fb_item.empty()) S.hy_fb_item.assign(4, 0);
-        conic_detail::number_pieces(S.hy_fa_item, S.hy_fa_lvl, S.hy_fc_item, S.npart);
+        conic_detail::number_pieces(S.hy_fa_item, S.hy_fa_lvl, S.hy_fc_item, S.hy_fslots);
+        if (!conic_detail::combine_in_phase_b(S.hy_fa_item, S.hy_fa_lvl, S.hy_fc_item, S.hy_fb_item, S.hy_fb_lvl, S.hy_fb_cmb,
+                                              S.nnzL + nk, S.nnzL, true)) {
+            S.err = "internal: a split target of the hybrid factorisation is finished twice";
+            return false;
+        }
     }
     // ---- substitutions: (node, entry range) runs per level ----
     {
@@ -749,8 +827,11 @@ inline bool cone_symbolic_build_hybrid(ConeSymbolic &S, int cut)
         }
         emit(fr, S.hy_fwp_item, S.hy_fwp_lvl, S.hy_fwp_R);
         emit(br, S.hy_bwp_item, S.hy_bwp_lvl, S.hy_bwp_R);
-        conic_detail::number_pieces(S.hy_fwp_item, S.hy_fwp_lvl, S.hy_fwc_item, S.npart);
-        conic_detail::number_pieces(S.hy_bwp_item, S.hy_bwp_lvl, S.hy_bwc_item, S.npart);
+        int fw_ = 0, bw_ = 0;
+        conic_detail::number_pieces(S.hy_fwp_item, S.hy_fwp_lvl, S.hy_fwc_item, fw_);
+        conic_detail::number_pieces(S.hy_bwp_item, S.hy_bwp_lvl, S.hy_bwc_item, bw_);
+        S.hy_sslots = std::max(fw_, bw_);
+        S.npart = std::max(S.npart, std::max(S.hy_fslots, S.hy_sslots));
     }
     // ---- top supernodes: descriptors in level order, update scatter lists as target ids ----
     {
