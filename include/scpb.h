@@ -194,6 +194,32 @@ int32_t scpb_ptr_free(scpb_ptr s);
  * e.g. the next step of a homotopy on a constraint-pack parameter (the reference sets mdl.traj.kappa between two
  * PTR.solve calls on one problem, test/examples/rendezvous_planar/tests.jl:66-78). */
 int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar);
+/* In-loop homotopy schedule (PTR only): the device twin of a problem_set_callback! that steps a constraint-pack parameter
+ * kappa through a grid inside ONE solve (test/examples/rendezvous_3d/definition.jl:96-151, called at ptr.jl:496-506).
+ * Every seed keeps its own grid index, kappa, last_update, effective iter_max and update threshold beta.  Right after the
+ * stopping rule of iteration `iter`, a seed whose subproblem solved safely updates when
+ *   beta >= improv_rel >= worsen_tol  and  its grid index < n_grid - 1   (false for a NaN improv_rel, as at iteration 1):
+ * kappa takes the next grid value, iter_max grows by iter - last_update, last_update = iter, and a stop the stopping rule
+ * asked for in that iteration is cancelled.  A seed ends with status 1 once iter >= its own iter_max.  Every solve starts
+ * every seed from grid[0], last_update = 1 and the descriptor's iter_max (the reference carries the mutated iter_max and
+ * kappa over to the next PTR.create on the same parameters).
+ * scpb_ptr_set_homotopy attaches the schedule to the homotopy parameter of the problem's constraint pack, which reads it
+ * from par[par_index] (the rendezvous pack's kappa, par[7]); par_index = -1 takes the pack's own slot, any other value
+ * must name it.  SCPB_ERR_UNSUPPORTED for a pack without a homotopy parameter.  n_grid = 0 detaches the schedule; an
+ * unchanged grid is not uploaded again.  A problem with a schedule refuses scpb_scvx_attach / scpb_gusto_attach and
+ * vice versa.  Streamed chains (SCPB_PTR_CHUNKS > 1) do not pay off with a schedule: the host polls every chain's
+ * progress (one core busy for the whole solve), and on the planar rendezvous beta sweep they ran at about half the
+ * lock-step rate.
+ * scpb_ptr_set_homotopy_beta sets beta[B] for the next solves, which must have B seeds.
+ * scpb_ptr_homotopy_result (after a solve with a schedule, same B): the final grid index hom_index[B], the effective
+ * iter_max_eff[B], and per iteration the grid index the subproblem was built with, hist_index[B][cap], and its
+ * improv_rel, hist_improv[B][cap]; -1 / NaN after a seed's last iteration.  A seed runs at most
+ * iter_max + (n_grid - 1)(iter_max - 1) iterations, so that many columns hold its whole history.  Every pointer is
+ * nullable. */
+int32_t scpb_ptr_set_homotopy(scpb_ptr s, int32_t par_index, int32_t n_grid, const double *grid, double worsen_tol);
+int32_t scpb_ptr_set_homotopy_beta(scpb_ptr s, int32_t B, const double *beta);
+int32_t scpb_ptr_homotopy_result(scpb_ptr s, int32_t B, int32_t *hom_index, int32_t *iter_max_eff, int32_t cap,
+                                 int32_t *hist_index, double *hist_improv);
 /* host arrays: initial guesses xd0[B][N][nx], ud0[B][N][nu], p0[B][np]; outputs the final iterates, per-seed
  * status (0 = stopping criterion met, 1 = iter_max reached [the reference still reports SCP_SOLVED],
  * 2+16*cone_status = SCP_FAILED), iteration counts, J_aug, deviation, dynamic feasibility flags and

@@ -140,6 +140,27 @@ ptr_set_par(h::Handle, ptr, par::Vector{Float64}) =
     check(h, ccall((:scpb_ptr_set_par, libscpb), Int32, (Ptr{Cvoid}, Ptr{Float64}, Int32), ptr, par, length(par)),
           "scpb_ptr_set_par")
 
+# scpb_ptr_set_homotopy / _beta / scpb_ptr_homotopy_result: the in-loop homotopy schedule that replaces a
+# problem_set_callback! stepping the pack's kappa through `grid` inside one solve (rendezvous_3d/definition.jl:96-151).
+# par_index is 0-based (the rendezvous pack's kappa is par[7]; -1 takes the pack's own slot); an empty grid detaches it.  The history
+# matrices are cap x B in Julia's column-major layout (the C ABI's [B][cap]).
+ptr_set_homotopy(h::Handle, ptr, par_index::Integer, grid::Vector{Float64}, worsen_tol::Float64 = -1e-3) =
+    check(h, ccall((:scpb_ptr_set_homotopy, libscpb), Int32, (Ptr{Cvoid}, Int32, Int32, Ptr{Float64}, Float64),
+                   ptr, par_index, length(grid), grid, worsen_tol), "scpb_ptr_set_homotopy")
+
+ptr_set_homotopy_beta(h::Handle, ptr, beta::Vector{Float64}) =
+    check(h, ccall((:scpb_ptr_set_homotopy_beta, libscpb), Int32, (Ptr{Cvoid}, Int32, Ptr{Float64}),
+                   ptr, length(beta), beta), "scpb_ptr_set_homotopy_beta")
+
+function ptr_homotopy_result(h::Handle, ptr, B::Integer, cap::Integer)
+    hom_index = Vector{Int32}(undef, B); iter_max = Vector{Int32}(undef, B)
+    hist_index = Matrix{Int32}(undef, cap, B); hist_improv = Matrix{Float64}(undef, cap, B)
+    check(h, ccall((:scpb_ptr_homotopy_result, libscpb), Int32,
+        (Ptr{Cvoid}, Int32, Ptr{Int32}, Ptr{Int32}, Int32, Ptr{Int32}, Ptr{Float64}),
+        ptr, B, hom_index, iter_max, cap, hist_index, hist_improv), "scpb_ptr_homotopy_result")
+    return hom_index, iter_max, hist_index, hist_improv
+end
+
 # scpb_gusto_attach / scpb_gusto_solve (GuSTO.solve for a batch, src/solvers/gusto.jl:425-502, pen = :quad)
 struct GustoDesc
     lam_init::Float64; lam_max::Float64; rho_0::Float64; rho_1::Float64; beta_sh::Float64; beta_gr::Float64

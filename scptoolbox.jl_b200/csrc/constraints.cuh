@@ -7,6 +7,7 @@
 // has np = 1 + 6N parameters of which only the six room-SDF slacks of node k enter s at that node
 // (freeflyer/definition.jl:398-424), so its G has six columns instead of 481.
 #pragma once
+#include <type_traits>
 #include <math_constants.h>
 #include "models.cuh"
 
@@ -14,6 +15,21 @@ template <int ID>
 struct Constr {
     static constexpr int NS = 0;
 };
+
+// parameter slot of a pack's homotopy parameter (its KAPPA), or -1 for a pack without one
+template <class CP, class = void>
+struct HomSlot { static constexpr int value = -1; };
+template <class CP>
+struct HomSlot<CP, std::void_t<decltype(CP::KAPPA)>> { static constexpr int value = CP::KAPPA; };
+
+// the pack at node k; a pack with a homotopy parameter takes it from *kap (a seed's own value) unless kap is null
+template <class CP>
+__device__ __forceinline__ void constr_eval(const ModelPar &P, const double *kap, double t, int N, int k, const double *x,
+                                            const double *u, const double *p, double *s, double *C, double *D, double *G)
+{
+    if constexpr (HomSlot<CP>::value >= 0) CP::eval_kappa(P, kap ? *kap : P.v[CP::KAPPA], t, N, k, x, u, p, s, C, D, G);
+    else CP::eval(P, t, N, k, x, u, p, s, C, D, G);
+}
 
 // starship_flip/definition.jl:704-810.  par: [9] rate_delay, [10] deltadot_max, [11] gamma_gs, [12] thetamax2,
 // [8] tau_s (shared with the dynamics pack).
@@ -134,9 +150,11 @@ struct Constr<SCPB_MODEL_FREEFLYER> {
 // (kappa ~ 4.6e3) sigma = 1 - 1/(1 + exp(kappa L)) rounds to exactly 1 and the gradient factor
 // c = exp(kappa L + 2 log(1 - sigma)) to exactly 0, and a rearranged formula would not saturate on the same inputs.
 // par: m, J, lu, lv, n (dynamics pack) [0..4], then f_db [5], f_max [6], kappa [7].
+// KAPPA names the slot of the homotopy parameter: eval_kappa takes kappa as an argument, so the PTR loop can pass each
+// seed's own value of an in-loop homotopy schedule (scpb_ptr_set_homotopy) without copying the parameter block.
 template <>
 struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
-    static constexpr int NS = 6, NX = 6, NU = 12, NG = 1;
+    static constexpr int NS = 6, NX = 6, NU = 12, NG = 1, KAPPA = 7;
     __device__ static constexpr int gcol(int, int j) { return j; }
     // sigmoid([f0, f1], [g0, g1]; kappa) of two scalar predicates with scalar gradients: value sg, gradient dsg
     __device__ __forceinline__ static void sigmoid2(double f0, double f1, double g0, double g1, double kap, double &sg,
@@ -152,10 +170,15 @@ struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
         const double c = exp(__dadd_rn(kL, __dmul_rn(2.0, log(__dsub_rn(1.0, sg)))));
         dsg = __dmul_rn(__dmul_rn(kap, c), dL);
     }
-    __device__ static void eval(const ModelPar &P, double, int, int, const double *, const double *u, const double *,
-                                double *s, double *C, double *D, double *G)
+    __device__ static void eval(const ModelPar &P, double t, int N, int k, const double *x, const double *u,
+                                const double *p, double *s, double *C, double *D, double *G)
     {
-        const double fdb = P.v[5], fmx = P.v[6], kap = P.v[7];
+        eval_kappa(P, P.v[KAPPA], t, N, k, x, u, p, s, C, D, G);
+    }
+    __device__ static void eval_kappa(const ModelPar &P, double kap, double, int, int, const double *, const double *u,
+                                      const double *, double *s, double *C, double *D, double *G)
+    {
+        const double fdb = P.v[5], fmx = P.v[6];
         const double nrm = __dadd_rn(fmx, fdb);
         for (int i = 0; i < NS * NX; i++) C[i] = 0.0;
         for (int i = 0; i < NS * NU; i++) D[i] = 0.0;

@@ -9,7 +9,9 @@
 // Seeds that have stopped are frozen (their iterate is re-extracted unchanged) so a finished or failed
 // seed never stalls the batch.
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
+#include <thread>
 #include "handle.cuh"
 #include "discretize.cuh"
 #include "constraints.cuh"
@@ -38,6 +40,7 @@ struct PtrDev {
     int oeta = 0;
     const double *lam = nullptr;   // GuSTO: per-seed soft-penalty weight lambda, written to source olam (gusto.jl:228)
     int olam = 0;
+    const double *kappa = nullptr; // in-loop homotopy schedule: per-seed value of the pack's homotopy parameter
     int b0 = 0, nb = 0;            // chunk of seeds [b0, b0 + nb) of this launch (nb = 0: all B)
 };
 
@@ -60,7 +63,7 @@ __global__ void k_linearize(const PtrDev d, const double *xd, const double *ud, 
     if constexpr (CP::NS > 0) {
         constexpr int NS = CP::NS, NX = CP::NX, NU = CP::NU, NG = CP::NG;
         double s[NS], C[NS * NX], D[NS * NU], Gm[NS * NG];
-        CP::eval(d.par, d.t_grid[k], d.N, k, x, u, pp, s, C, D, Gm);
+        constr_eval<CP>(d.par, d.kappa ? d.kappa + b : nullptr, d.t_grid[k], d.N, k, x, u, pp, s, C, D, Gm);
         for (int r = 0; r < NS; r++) {
             double rs = s[r];
             for (int j = 0; j < NX; j++) { rs -= C[r * NX + j] * x[j]; d.src[gaddr(b, G, E, d.oC + ((long long)k * NS + r) * NX + j)] = C[r * NX + j]; }
@@ -125,6 +128,17 @@ struct StepDev {
     double *J_ref, *J_new, *dev, *imp;
     const int *feas_new;
     int *done, *status, *iters, *nactive;
+    // in-loop homotopy schedule (scpb_ptr_set_homotopy; hom_n = 0: none), the device twin of the reference's callback
+    // (rendezvous_3d/definition.jl:96-151, called at ptr.jl:496-506): per seed the grid index, the homotopy parameter,
+    // the iteration of the last update, the effective iter_max and the update threshold beta
+    int hom_n = 0, hist_cap = 0;
+    double worsen_tol = 0.0;
+    const double *hom_grid = nullptr, *hom_beta = nullptr;
+    int *hom_idx = nullptr, *hom_last = nullptr, *hom_itmax = nullptr;
+    double *hom_kappa = nullptr;
+    int *hist_idx = nullptr;       // [B][hist_cap]: grid index each iteration's subproblem was built with ...
+    double *hist_imp = nullptr;    // ... and its improv_rel
+    int *ndone = nullptr;          // streamed loop with a schedule: seeds of this chunk that have finished
 };
 
 // extract the new iterate (physical units) for active seeds; frozen seeds re-emit their accepted iterate
@@ -169,8 +183,10 @@ __global__ void k_ptr_step(const StepDev d)
     if (d.done[b]) return;
     if (d.ipm_total) atomicAdd(d.ipm_total, (unsigned long long)d.cone_iters[b]);
     const int cs = d.cone_status[b];
-    if (!(cs == IPM_OPTIMAL || cs == IPM_ALMOST)) {  // unsafe_solution, scp.jl:965-980
+    if (d.hom_n > 0) d.hist_idx[(size_t)b * d.hist_cap + d.iter - 1] = d.hom_idx[b];
+    if (!(cs == IPM_OPTIMAL || cs == IPM_ALMOST)) {  // unsafe_solution, scp.jl:965-980: before the callback (ptr.jl:488-491)
         d.done[b] = 1; d.status[b] = 2 + 16 * cs; d.iters[b] = d.iter;
+        if (d.ndone) atomicAdd(d.ndone, 1);
         return;
     }
     const int q = d.q_exit;
@@ -192,6 +208,21 @@ __global__ void k_ptr_step(const StepDev d)
     const double imp = (Jr - Jn) / fabs(Jr);
     d.dev[b] = deviation; d.imp[b] = imp;
     const bool stop = d.iter > 1 && d.feas_new[b] && (fabs(imp) <= d.eps_rel || deviation <= d.eps_abs);
+    // the schedule's update: the next grid value when improv_rel lies in [worsen_tol, beta] and the grid is not exhausted
+    // (false for a NaN improv_rel, as at iteration 1); iter_max then grows by the iterations since the last update, and
+    // a stop the stopping rule asked for in this iteration is cancelled (ptr.jl:496-506)
+    bool acted = false;
+    if (d.hom_n > 0) {
+        d.hist_imp[(size_t)b * d.hist_cap + d.iter - 1] = imp;
+        const int idx = d.hom_idx[b];
+        acted = imp <= d.hom_beta[b] && imp >= d.worsen_tol && idx < d.hom_n - 1;
+        if (acted) {
+            d.hom_idx[b] = idx + 1;
+            d.hom_kappa[b] = d.hom_grid[idx + 1];
+            d.hom_itmax[b] += d.iter - d.hom_last[b];
+            d.hom_last[b] = d.iter;
+        }
+    }
     // accept: ref <- sol
     for (int k = 0; k < d.N; k++) {
         for (int j = 0; j < d.nx; j++) { const size_t o = ((size_t)b * d.N + k) * d.nx + j; d.xd[o] = d.xn[o]; }
@@ -200,8 +231,24 @@ __global__ void k_ptr_step(const StepDev d)
     for (int j = 0; j < d.np; j++) d.p[(size_t)b * d.np + j] = d.pn[(size_t)b * d.np + j];
     d.J_ref[b] = Jn;
     d.iters[b] = d.iter;
-    if (stop) { d.done[b] = 1; d.status[b] = 0; }
-    else atomicAdd(d.nactive, 1);
+    if (stop && !acted) {
+        d.done[b] = 1; d.status[b] = 0;
+        if (d.ndone) atomicAdd(d.ndone, 1);
+    } else if (d.hom_n > 0 && d.iter >= d.hom_itmax[b]) {   // the seed's own iter_max: status stays 1
+        d.done[b] = 1;
+        if (d.ndone) atomicAdd(d.ndone, 1);
+    } else atomicAdd(d.nactive, 1);
+}
+
+// start of a solve with a schedule: every seed from grid[0], the configured iter_max and last_update = 1 (the
+// reference's default when the reference solution carries no update yet); history cleared to -1 / NaN
+__global__ void k_hom_init(const StepDev d, int iter_max, int nB)
+{
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < nB) {
+        d.hom_idx[i] = 0; d.hom_kappa[i] = d.hom_grid[0]; d.hom_last[i] = 1; d.hom_itmax[i] = iter_max;
+    }
+    if (i < (long long)nB * d.hist_cap) { d.hist_idx[i] = -1; d.hist_imp[i] = CUDART_NAN; }
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -242,6 +289,18 @@ struct scpb_ptr_s {
     // streamed PTR loop (scpb_ptr_solve): one stream per chunk of seed groups, device counter of interior-point iterations
     std::vector<cudaStream_t> chunk_streams;
     unsigned long long *d_ipm_total = nullptr;
+    // in-loop homotopy schedule (scpb_ptr_set_homotopy): grid, threshold per seed, state and history of the last solve
+    int hom_n = 0, hom_slot = -1, hom_cap = 0;   // hom_cap: history columns = the longest chain a seed can run
+    double hom_wtol = 0.0;
+    double *hom_grid = nullptr;
+    std::vector<double> hom_grid_h;               // host copy of the device grid: an unchanged grid is not re-uploaded
+    std::vector<double> hom_beta_h;               // scpb_ptr_set_homotopy_beta: one per seed of the next solves
+    std::vector<void *> hb;                       // per-seed buffers below, sized for hom_capB seeds x hom_cap
+    int hom_capB = 0, hom_bufcap = 0, last_B = 0, last_cap = 0;   // last_cap: history columns of the last solve (0: none)
+    double *hom_beta = nullptr, *hom_kappa = nullptr, *hist_imp = nullptr;
+    int *hom_idx = nullptr, *hom_last = nullptr, *hom_itmax = nullptr, *hist_idx = nullptr;
+    int *d_chunk_done = nullptr, *h_chunk_done = nullptr;   // streamed loop: finished seeds per chunk (device, pinned copy)
+    int chunk_cap = 0;
 };
 
 // the handle may have been pointed at another model pack since scpb_ptr_setup (several problems can share one handle):
@@ -342,6 +401,32 @@ static int ptr_reserve(scpb_ptr_s *s, int B, int G)
     }
     if (!ok) { cudaGetLastError(); drop(); return set_err(h, SCPB_ERR_CUDA, "ptr: device allocation failed (B=%d)", B); }
     s->capB = Bpad; s->capG = G;
+    return SCPB_OK;
+}
+
+// the schedule's per-seed state and history for Bpad seeds
+static int hom_reserve(scpb_ptr_s *s, int Bpad)
+{
+    if (s->hom_capB >= Bpad && s->hom_bufcap >= s->hom_cap) return SCPB_OK;
+    for (void *q : s->hb) if (q) cudaFree(q);
+    s->hb.clear();
+    s->hom_capB = 0; s->hom_bufcap = 0;
+    s->hom_beta = s->hom_kappa = s->hist_imp = nullptr;
+    s->hom_idx = s->hom_last = s->hom_itmax = s->hist_idx = nullptr;
+    bool ok = true;
+    auto al = [&](size_t bytes) { void *q = nullptr; if (cudaMalloc(&q, bytes + 64) != cudaSuccess) { ok = false; return (void *)nullptr; } s->hb.push_back(q); return q; };
+    const size_t H = (size_t)Bpad * s->hom_cap;
+    s->hom_beta = (double *)al(sizeof(double) * Bpad); s->hom_kappa = (double *)al(sizeof(double) * Bpad);
+    s->hom_idx = (int *)al(sizeof(int) * Bpad); s->hom_last = (int *)al(sizeof(int) * Bpad);
+    s->hom_itmax = (int *)al(sizeof(int) * Bpad);
+    s->hist_idx = (int *)al(sizeof(int) * H); s->hist_imp = (double *)al(sizeof(double) * H);
+    if (!ok) {
+        cudaGetLastError();
+        for (void *q : s->hb) if (q) cudaFree(q);
+        s->hb.clear();
+        return set_err(s->h, SCPB_ERR_CUDA, "ptr: device allocation of the homotopy state failed (B=%d)", Bpad);
+    }
+    s->hom_capB = Bpad; s->hom_bufcap = s->hom_cap;
     return SCPB_OK;
 }
 
@@ -713,8 +798,8 @@ __global__ void k_debug_constr(const ModelPar par, int B, int N, const double *t
     if (i >= (long long)B * N) return;
     const int b = (int)(i / N), k = (int)(i % N);
     constexpr int NS = CP::NS, NX = CP::NX, NU = CP::NU, NG = CP::NG;
-    CP::eval(par, t_grid[k], N, k, xd + (size_t)i * NX, ud + (size_t)i * NU, p + (size_t)b * np, s + (size_t)i * NS,
-             C + (size_t)i * NS * NX, D + (size_t)i * NS * NU, G + (size_t)i * NS * NG);
+    constr_eval<CP>(par, nullptr, t_grid[k], N, k, xd + (size_t)i * NX, ud + (size_t)i * NU, p + (size_t)b * np,
+                    s + (size_t)i * NS, C + (size_t)i * NS * NX, D + (size_t)i * NS * NU, G + (size_t)i * NS * NG);
 }
 
 template <class CP>
@@ -870,6 +955,87 @@ int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar)
     return SCPB_OK;
 }
 
+// parameter slot of the homotopy parameter of a model's constraint pack (HomSlot, csrc/constraints.cuh), -1: none
+static int pack_hom_slot(int model_id)
+{
+    switch (model_id) {
+    case SCPB_MODEL_STARSHIP: return HomSlot<Constr<SCPB_MODEL_STARSHIP>>::value;
+    case SCPB_MODEL_QUADROTOR: return HomSlot<Constr<SCPB_MODEL_QUADROTOR>>::value;
+    case SCPB_MODEL_FREEFLYER: return HomSlot<Constr<SCPB_MODEL_FREEFLYER>>::value;
+    case SCPB_MODEL_RENDEZVOUS2D: return HomSlot<Constr<SCPB_MODEL_RENDEZVOUS2D>>::value;
+    default: return -1;
+    }
+}
+
+int32_t scpb_ptr_set_homotopy(scpb_ptr s, int32_t par_index, int32_t n_grid, const double *grid, double worsen_tol)
+{
+    if (!s) return SCPB_ERR_ARG;
+    scpb_handle_s *h = s->h;
+    if (n_grid == 0) { s->hom_n = 0; s->hom_cap = 0; s->hom_slot = -1; s->hom_grid_h.clear(); return SCPB_OK; }
+    if (n_grid < 0 || !grid) return set_err(h, SCPB_ERR_ARG, "ptr_set_homotopy: n_grid = %d with grid %p", n_grid, grid);
+    if (s->scvx || s->gusto) return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_set_homotopy: schedules are implemented for PTR only");
+    const int slot = s->d.ns > 0 ? pack_hom_slot(s->model_id) : -1;
+    if (slot < 0 || (par_index >= 0 && slot != par_index))
+        return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_set_homotopy: the constraint pack of model %d does not read a homotopy "
+                       "parameter at par[%d]", s->model_id, par_index);
+    for (int i = 0; i < n_grid; i++)
+        if (!std::isfinite(grid[i])) return set_err(h, SCPB_ERR_ARG, "ptr_set_homotopy: grid[%d] is not finite", i);
+    if (std::isnan(worsen_tol)) return set_err(h, SCPB_ERR_ARG, "ptr_set_homotopy: worsen_tol is NaN");
+    s->hom_slot = slot; s->hom_wtol = worsen_tol;
+    s->hom_cap = s->d.iter_max + (n_grid - 1) * std::max(s->d.iter_max - 1, 0);
+    if (s->hom_n == n_grid && std::equal(grid, grid + n_grid, s->hom_grid_h.begin())) return SCPB_OK;   // same grid
+    SCPB_CUDA(h, cudaSetDevice(h->device));
+    // the grid may still be read by a solve queued on the stream
+    SCPB_CUDA(h, cudaStreamSynchronize(h->stream));
+    if (s->hom_grid) cudaFree(s->hom_grid);
+    s->hom_grid = nullptr; s->hom_n = 0; s->hom_cap = 0; s->hom_grid_h.clear();
+    SCPB_CUDA(h, cudaMalloc((void **)&s->hom_grid, sizeof(double) * n_grid));
+    SCPB_CUDA(h, cudaMemcpy(s->hom_grid, grid, sizeof(double) * n_grid, cudaMemcpyHostToDevice));
+    s->hom_grid_h.assign(grid, grid + n_grid);
+    s->hom_n = n_grid;
+    s->hom_cap = s->d.iter_max + (n_grid - 1) * std::max(s->d.iter_max - 1, 0);
+    return SCPB_OK;
+}
+
+int32_t scpb_ptr_set_homotopy_beta(scpb_ptr s, int32_t B, const double *beta)
+{
+    if (!s) return SCPB_ERR_ARG;
+    if (B <= 0 || !beta) return set_err(s->h, SCPB_ERR_ARG, "ptr_set_homotopy_beta: bad arguments (B = %d)", B);
+    for (int b = 0; b < B; b++)
+        if (std::isnan(beta[b])) return set_err(s->h, SCPB_ERR_ARG, "ptr_set_homotopy_beta: beta[%d] is NaN", b);
+    s->hom_beta_h.assign(beta, beta + B);
+    return SCPB_OK;
+}
+
+int32_t scpb_ptr_homotopy_result(scpb_ptr s, int32_t B, int32_t *hom_index, int32_t *iter_max_eff, int32_t cap,
+                                 int32_t *hist_index, double *hist_improv)
+{
+    if (!s) return SCPB_ERR_ARG;
+    scpb_handle_s *h = s->h;
+    if (s->last_cap == 0) return set_err(h, SCPB_ERR_STATE, "ptr_homotopy_result: the last solve had no schedule");
+    if (B != s->last_B) return set_err(h, SCPB_ERR_ARG, "ptr_homotopy_result: the last solve had %d seeds, not %d", s->last_B, B);
+    if (cap < 0 || ((hist_index || hist_improv) && cap == 0))
+        return set_err(h, SCPB_ERR_ARG, "ptr_homotopy_result: cap = %d", cap);
+    SCPB_CUDA(h, cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    if (hom_index) SCPB_CUDA(h, cudaMemcpyAsync(hom_index, s->hom_idx, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    if (iter_max_eff) SCPB_CUDA(h, cudaMemcpyAsync(iter_max_eff, s->hom_itmax, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    const int w = std::min(cap, s->last_cap);
+    if (hist_index)
+        SCPB_CUDA(h, cudaMemcpy2DAsync(hist_index, sizeof(int) * cap, s->hist_idx, sizeof(int) * s->last_cap, sizeof(int) * w,
+                                       B, cudaMemcpyDeviceToHost, st));
+    if (hist_improv)
+        SCPB_CUDA(h, cudaMemcpy2DAsync(hist_improv, sizeof(double) * cap, s->hist_imp, sizeof(double) * s->last_cap,
+                                       sizeof(double) * w, B, cudaMemcpyDeviceToHost, st));
+    SCPB_CUDA(h, cudaStreamSynchronize(st));
+    for (int b = 0; b < B; b++)
+        for (int j = w; j < cap; j++) {
+            if (hist_index) hist_index[(size_t)b * cap + j] = -1;
+            if (hist_improv) hist_improv[(size_t)b * cap + j] = nan("");
+        }
+    return SCPB_OK;
+}
+
 int32_t scpb_ptr_free(scpb_ptr s)
 {
     if (!s) return SCPB_ERR_ARG;
@@ -879,6 +1045,10 @@ int32_t scpb_ptr_free(scpb_ptr s)
     for (void *q : s->bb) if (q) cudaFree(q);
     for (cudaStream_t q : s->chunk_streams) if (q) cudaStreamDestroy(q);
     if (s->d_ipm_total) cudaFree(s->d_ipm_total);
+    for (void *q : s->hb) if (q) cudaFree(q);
+    if (s->hom_grid) cudaFree(s->hom_grid);
+    if (s->d_chunk_done) cudaFree(s->d_chunk_done);
+    if (s->h_chunk_done) cudaFreeHost(s->h_chunk_done);
     delete s;
     return SCPB_OK;
 }
@@ -898,6 +1068,16 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
     int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
     if (rc) return rc;
     if ((rc = ptr_reserve(s, B, G))) return rc;
+    const bool hom = s->hom_n > 0;
+    if (hom) {
+        if ((int)s->hom_beta_h.size() != B)
+            return set_err(h, SCPB_ERR_STATE, "ptr_solve: the homotopy schedule has %d update thresholds for %d seeds "
+                           "(scpb_ptr_set_homotopy_beta)", (int)s->hom_beta_h.size(), B);
+        if ((rc = hom_reserve(s, s->capB))) return rc;
+    }
+    // a seed with a schedule can run iter_max + (n_grid - 1)(iter_max - 1) iterations (every update extends its
+    // iter_max by the iterations since the previous one)
+    const int it_bound = hom ? s->hom_cap : d.iter_max;
     IpmData *D = scpb_internal_cone_data(s->cone);
     const ConeSymbolic *S = scpb_internal_cone_sym(s->cone);
     IpmOpts o_ = scpb_internal_make_opts(opts);
@@ -937,6 +1117,18 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
     sd.xd = s->xd; sd.ud = s->ud; sd.p = s->p; sd.xn = s->xn; sd.un = s->un; sd.pn = s->pn;
     sd.J_ref = s->J_ref; sd.J_new = s->J_new; sd.dev = s->devi; sd.imp = s->imp; sd.feas_new = s->feas;
     sd.done = s->done; sd.status = s->status; sd.iters = s->iters; sd.nactive = s->nactive;
+    s->last_B = B; s->last_cap = hom ? s->hom_cap : 0;
+    if (hom) {
+        pd.kappa = s->hom_kappa;
+        sd.hom_n = s->hom_n; sd.hist_cap = s->hom_cap; sd.worsen_tol = s->hom_wtol;
+        sd.hom_grid = s->hom_grid; sd.hom_beta = s->hom_beta;
+        sd.hom_idx = s->hom_idx; sd.hom_last = s->hom_last; sd.hom_itmax = s->hom_itmax; sd.hom_kappa = s->hom_kappa;
+        sd.hist_idx = s->hist_idx; sd.hist_imp = s->hist_imp;
+        SCPB_CUDA(h, cudaMemcpyAsync(s->hom_beta, s->hom_beta_h.data(), sizeof(double) * B, cudaMemcpyHostToDevice, st));
+        const long long n_init = (long long)B * s->hom_cap;
+        k_hom_init<<<(unsigned)((n_init + 127) / 128), 128, 0, st>>>(sd, d.iter_max, B);
+        h->launches++;
+    }
 
     // phase timers (the reference's keys: discretize / formulate / solve / overhead, scp.jl:177-178,990-995)
     EventList evl;
@@ -986,34 +1178,86 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
         for (int c = 0; c < n_chunks; c++) SCPB_CUDA(h, cudaStreamWaitEvent(s->chunk_streams[c], e_fork, 0));
         auto mark0 = [&](int ph) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s->chunk_streams[0]); ev.push_back(e); phase.push_back(ph); };
         mark0(-1);   // chunk 0 carries the phase timers: its own chain is one of the n_chunks concurrent critical paths
-        for (it = 1; it <= d.iter_max; it++) {
-            for (int c = 0; c < n_chunks; c++) {
-                cudaStream_t cs = s->chunk_streams[c];
-                const int b0 = c * cg * G;
-                const int nbp = std::min(cg * G, Bpad - b0), nb = std::min(nbp, B - b0);
-                if (nb <= 0) continue;
-                const int nbn_c = (int)(((long long)nb * d.N + 127) / 128);
-                pd.b0 = b0; pd.nb = nb;
-                launch_linearize(s, pd, nbn_c, cs);
-                ad.b0 = b0; ad.nbp = nbp;
-                k_assemble<<<(unsigned)(((long long)d.nval * nbp + 255) / 256), 256, 0, cs>>>(ad);
-                h->launches += 2;
-                if (c == 0) mark0(1);
-                {
-                    IpmOpts ow = o;
-                    ow.warm = (it >= warm_from && !no_warm) ? 1 : 0;
-                    if ((rc = scpb_internal_cone_run(s->cone, ow, s->done, cs, b0 / G, nbp / G))) return rc;
+        // iteration `it` of chunk c's chain
+        auto enqueue = [&](int c, int it) -> int {
+            cudaStream_t cs = s->chunk_streams[c];
+            const int b0 = c * cg * G;
+            const int nbp = std::min(cg * G, Bpad - b0), nb = std::min(nbp, B - b0);
+            const int nbn_c = (int)(((long long)nb * d.N + 127) / 128);
+            pd.b0 = b0; pd.nb = nb;
+            launch_linearize(s, pd, nbn_c, cs);
+            ad.b0 = b0; ad.nbp = nbp;
+            k_assemble<<<(unsigned)(((long long)d.nval * nbp + 255) / 256), 256, 0, cs>>>(ad);
+            h->launches += 2;
+            if (c == 0) mark0(1);
+            {
+                IpmOpts ow = o;
+                ow.warm = (it >= warm_from && !no_warm) ? 1 : 0;
+                if (int r = scpb_internal_cone_run(s->cone, ow, s->done, cs, b0 / G, nbp / G)) return r;
+            }
+            if (c == 0) mark0(2);
+            sd.iter = it; sd.b0 = b0; sd.nb = nb;
+            sd.ndone = hom ? s->d_chunk_done + c : nullptr;
+            k_extract<<<nbn_c, 128, 0, cs>>>(sd);
+            h->launches++;
+            if (c == 0) mark0(3);
+            if (int r = run_discretize(s, B, G, s->xn, s->un, s->pn, nullptr, s->done, cs, b0, nb)) return r;
+            if (c == 0) mark0(0);
+            k_ptr_step<<<(nb + 127) / 128, 128, 0, cs>>>(sd);
+            h->launches++;
+            if (c == 0) mark0(3);
+            return SCPB_OK;
+        };
+        auto chunk_seeds = [&](int c) { const int b0 = c * cg * G; return std::min(std::min(cg * G, Bpad - b0), B - b0); };
+        if (!hom) {
+            for (it = 1; it <= it_bound; it++)
+                for (int c = 0; c < n_chunks; c++)
+                    if (chunk_seeds(c) > 0 && (rc = enqueue(c, it))) return rc;
+        } else {
+            // A schedule lets a seed run up to it_bound iterations, but most chains end far earlier.  Every chain keeps at
+            // most LAG iterations queued: before iteration j it waits (without blocking the other chains) for the event
+            // of iteration j - LAG and reads its chunk's count of finished seeds, copied to pinned memory after every
+            // k_ptr_step.  The count only grows, so a stale value can only delay a chain's end by LAG empty iterations.
+            constexpr int LAG = 3;
+            if (s->chunk_cap < n_chunks) {
+                if (s->d_chunk_done) cudaFree(s->d_chunk_done);
+                if (s->h_chunk_done) cudaFreeHost(s->h_chunk_done);
+                s->d_chunk_done = nullptr; s->h_chunk_done = nullptr; s->chunk_cap = 0;
+                SCPB_CUDA(h, cudaMalloc((void **)&s->d_chunk_done, sizeof(int) * n_chunks));
+                SCPB_CUDA(h, cudaMallocHost((void **)&s->h_chunk_done, sizeof(int) * n_chunks));
+                s->chunk_cap = n_chunks;
+            }
+            SCPB_CUDA(h, cudaMemsetAsync(s->d_chunk_done, 0, sizeof(int) * n_chunks, st));
+            for (int c = 0; c < n_chunks; c++) s->h_chunk_done[c] = 0;
+            SCPB_CUDA(h, cudaEventRecord(e_fork, st));   // the chains also wait for the cleared counters
+            for (int c = 0; c < n_chunks; c++) SCPB_CUDA(h, cudaStreamWaitEvent(s->chunk_streams[c], e_fork, 0));
+            std::vector<cudaEvent_t> ring((size_t)n_chunks * LAG);
+            for (cudaEvent_t &e : ring) e = sync_event();
+            std::vector<int> next(n_chunks, 1), fin(n_chunks, 0);
+            int live = 0;
+            for (int c = 0; c < n_chunks; c++) { if (chunk_seeds(c) > 0) live++; else fin[c] = 1; }
+            volatile int *seen = s->h_chunk_done;
+            while (live > 0) {
+                bool moved = false;
+                for (int c = 0; c < n_chunks; c++) {
+                    if (fin[c]) continue;
+                    const int j = next[c];
+                    cudaEvent_t &e = ring[(size_t)c * LAG + j % LAG];   // recorded after iteration j - LAG
+                    if (j > it_bound) { fin[c] = 1; live--; continue; }
+                    if (j > LAG) {
+                        const cudaError_t q = cudaEventQuery(e);
+                        if (q == cudaErrorNotReady) continue;
+                        SCPB_CUDA(h, q);
+                        if (seen[c] >= chunk_seeds(c)) { fin[c] = 1; live--; continue; }
+                    }
+                    if ((rc = enqueue(c, j))) return rc;
+                    cudaStream_t cs = s->chunk_streams[c];
+                    SCPB_CUDA(h, cudaMemcpyAsync(s->h_chunk_done + c, s->d_chunk_done + c, sizeof(int), cudaMemcpyDeviceToHost, cs));
+                    SCPB_CUDA(h, cudaEventRecord(e, cs));
+                    next[c] = j + 1;
+                    moved = true;
                 }
-                if (c == 0) mark0(2);
-                sd.iter = it; sd.b0 = b0; sd.nb = nb;
-                k_extract<<<nbn_c, 128, 0, cs>>>(sd);
-                h->launches++;
-                if (c == 0) mark0(3);
-                if ((rc = run_discretize(s, B, G, s->xn, s->un, s->pn, nullptr, s->done, cs, b0, nb))) return rc;
-                if (c == 0) mark0(0);
-                k_ptr_step<<<(nb + 127) / 128, 128, 0, cs>>>(sd);
-                h->launches++;
-                if (c == 0) mark0(3);
+                if (!moved) std::this_thread::yield();
             }
         }
         for (int c = 0; c < n_chunks; c++) {   // join
@@ -1029,10 +1273,10 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
         SCPB_CUDA(h, cudaStreamSynchronize(st));
         ipm_iters = (long long)tot_ipm;
         for (int b = 0; b < B; b++) total_it = std::max(total_it, hiters[b]);   // the longest chain
-        it = d.iter_max + 1;   // skip the lock-step loop
+        it = it_bound + 1;   // skip the lock-step loop
     }
     std::vector<int> hit(B), hdone(B, 0);   // hdone: seeds that were already finished when the solver was launched (skipped)
-    for (; it <= d.iter_max; it++) {
+    for (; it <= it_bound; it++) {
         launch_linearize(s, pd, nbn, st);
         const long long tot = (long long)d.nval * Bpad;
         k_assemble<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ad);
@@ -1100,6 +1344,7 @@ int32_t scpb_scvx_attach(scpb_ptr s, const scpb_scvx_desc *desc, const int32_t *
     scpb_handle_s *h = s->h;
     if (!desc || !Q_rowptr || !Q_colind || !Q_vals || !Q_const) return set_err(h, SCPB_ERR_ARG, "scvx_attach: null pointer");
     const scpb_ptr_desc &d = s->d;
+    if (s->hom_n > 0) return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: the problem has an in-loop homotopy schedule (PTR only)");
     if (d.method != SCPB_FOH) return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: SCvx runs with FOH discretization only");
     if (desc->oeta <= 0 || desc->oeta >= d.nsrc || desc->n_ic < 0 || desc->n_tc < 0)
         return set_err(h, SCPB_ERR_ARG, "scvx_attach: bad descriptor (oeta=%d)", desc->oeta);
@@ -1280,6 +1525,7 @@ int32_t scpb_gusto_attach(scpb_ptr s, const scpb_gusto_desc *desc, const int32_t
     if (!desc || !Q_rowptr || !Q_colind || !Q_vals || !Q_const || (desc->nsq > 0 && !Q_weight))
         return set_err(h, SCPB_ERR_ARG, "gusto_attach: null pointer");
     const scpb_ptr_desc &d = s->d;
+    if (s->hom_n > 0) return set_err(h, SCPB_ERR_UNSUPPORTED, "gusto_attach: the problem has an in-loop homotopy schedule (PTR only)");
     if (d.method != SCPB_FOH) return set_err(h, SCPB_ERR_UNSUPPORTED, "gusto_attach: GuSTO runs with FOH discretization only");
     if (desc->oeta <= 0 || desc->oeta >= d.nsrc || desc->olam <= 0 || desc->olam >= d.nsrc || desc->olam == desc->oeta ||
         desc->nsq < 0 || desc->q_tr < 0 || desc->q_tr > 2)

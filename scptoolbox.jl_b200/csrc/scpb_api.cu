@@ -93,7 +93,7 @@ static void julia_views(DiscArgs &a, int nx, int nu, int np, double *A, double *
 
 extern "C" {
 
-int32_t scpb_version(void) { return 101; }
+int32_t scpb_version(void) { return 102; }
 
 int32_t scpb_create(int32_t device, scpb_handle *out)
 {

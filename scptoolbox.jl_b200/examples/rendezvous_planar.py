@@ -8,7 +8,8 @@ test/examples/rendezvous_planar/definition.jl (dims :36-41, scaling advice :43-9
 State x = [r(2) v(2) theta omega], input u = [f(3) fr(3) l1f(3) l1feq(3)] (thrust of the three RCS pods, their reference
 values, |f| and |f - fr|), parameter p = [tdil].  Every variable carries scaling advice, so no bounding-box solve is
 needed.  The deadband constraint f = OR(fr) fr is a smooth OR whose sharpness kappa is stepped through a homotopy; each
-step is warm-started from the previous solution (homotopy_sweep)."""
+step is warm-started from the previous solution (homotopy_sweep), or stepped inside one solve by the in-loop schedule
+(homotopy_schedule, the pattern of test/examples/rendezvous_3d/definition.jl:96-151)."""
 from __future__ import annotations
 
 import math
@@ -19,7 +20,8 @@ from .. import lib, ptr
 from ..homotopy import Homotopy
 from ..parser import Expr
 from ..problem import (TrajectoryProblem, problem_advise_scale, problem_set_bc, problem_set_dims, problem_set_dynamics,
-                       problem_set_guess, problem_set_running_cost, problem_set_s, problem_set_U)
+                       problem_set_guess, problem_set_homotopy_update, problem_set_running_cost, problem_set_s,
+                       problem_set_U)
 
 ID_F, ID_FR, ID_L1F, ID_L1FEQ = range(0, 3), range(3, 6), range(6, 9), range(9, 12)
 
@@ -153,3 +155,11 @@ def homotopy_sweep(pbm, guesses=None, n_hom=10, hom=None, **cone_opts):
         warm = ptr.solve(pbm, warm, **cone_opts)
         sols.append(warm)
     return sols
+
+
+def homotopy_schedule(traj, beta, n_hom=10, hom=None, worsen_tol=-1e-3):
+    """Step kappa through hom(LinRange(0, 1, n_hom)) (default Homotopy(1e-3; delta_max = 5)) inside ONE PTR solve: a seed
+    moves to the next value when its relative cost improvement lies in [worsen_tol, beta] (problem_set_homotopy_update).
+    Call before ptr.create or between solves; ptr.solve(..., beta=[...]) then sweeps the threshold over a batch."""
+    hom = hom or Homotopy(1e-3, delta_max=5.0)
+    problem_set_homotopy_update(traj, [hom(x) for x in ptr.t_grid(n_hom)], beta, worsen_tol)

@@ -50,6 +50,9 @@ SIGNATURES = {
     "scpb_ptr_setup": (C.c_int32, [C.c_void_p, C.c_void_p, C.c_void_p, _ip, _ip, _dp, _dp, _dp, C.POINTER(C.c_void_p)]),
     "scpb_ptr_free": (C.c_int32, [C.c_void_p]),
     "scpb_ptr_set_par": (C.c_int32, [C.c_void_p, _dp, C.c_int32]),
+    "scpb_ptr_set_homotopy": (C.c_int32, [C.c_void_p, C.c_int32, C.c_int32, _dp, C.c_double]),
+    "scpb_ptr_set_homotopy_beta": (C.c_int32, [C.c_void_p, C.c_int32, _dp]),
+    "scpb_ptr_homotopy_result": (C.c_int32, [C.c_void_p, C.c_int32, _ip, _ip, C.c_int32, _ip, _dp]),
     "scpb_ptr_solve": (C.c_int32, [C.c_void_p, C.c_int32, _dp, _dp, _dp, C.c_void_p, _dp, _dp, _dp, _ip, _ip,
                                    _dp, _dp, _ip, _dp]),
     "scpb_scvx_attach": (C.c_int32, [C.c_void_p, C.c_void_p, _ip, _ip, _dp, _dp]),

@@ -36,6 +36,7 @@ class TrajectoryProblem:
         self.gic = None          # affine boundary conditions g(x_expr, p_expr, pbm) -> list[Expr]
         self.gtc = None
         self.scp = None
+        self.hom = None          # in-loop homotopy schedule (problem_set_homotopy_update)
 
 
 def problem_set_dims(pbm, nx, nu, np_):
@@ -128,6 +129,26 @@ def problem_advise_parameter_stage(pbm, stage_of):
     """GPU-specific ordering advice: stage_of(N) -> list (len np) with the time node a parameter is tied to, or
     -1 for a genuinely global parameter (used only for the elimination order of the KKT factorisation)."""
     pbm.p_stage = stage_of
+
+
+def problem_set_homotopy_update(pbm, grid, beta, worsen_tol=-1e-3, par_index=None):
+    """The declarative twin of a problem_set_callback! (problem.jl:645-659) that steps the constraint pack's homotopy
+    parameter through `grid` inside one PTR solve, as test/examples/rendezvous_3d/definition.jl:96-151 does.  After the
+    stopping rule of iteration `iter`, a seed updates when beta >= improv_rel >= worsen_tol and the grid is not
+    exhausted: the parameter takes the next grid value, iter_max grows by iter - last_update, and a stop asked for in
+    that iteration is cancelled.  Runs on the device, per seed (csrc/ptr.cu, k_ptr_step); every solve restarts each seed
+    from grid[0] and the configured iter_max.
+    beta: the default update threshold (ptr.solve(..., beta=...) overrides it per solve or per seed).
+    par_index: the parameter slot the pack reads the homotopy parameter from (None: the pack's own; the device refuses
+    any other slot).
+    grid = None removes the schedule."""
+    if grid is None:
+        pbm.hom = None
+        return
+    grid = np.ascontiguousarray(grid, dtype=np.float64).ravel()
+    if grid.size == 0 or not np.isfinite(grid).all():
+        raise ValueError("the homotopy grid must be a non-empty list of finite values")
+    pbm.hom = dict(grid=grid, beta=float(beta), worsen_tol=float(worsen_tol), par_index=par_index)
 
 
 def problem_set_bc(pbm, kind, g):

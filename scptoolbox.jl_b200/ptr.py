@@ -196,6 +196,8 @@ class SCPProblem:
         if pars.disc_method == IMPULSE and traj.model_id not in IMPULSE_MODELS:
             raise lib.ScpbError(f"IMPULSE discretization needs a model pack with impulse semantics (model {traj.model_id} "
                                 "has none)")
+        if getattr(traj, "hom", None) is not None and algo != "ptr":
+            raise lib.ScpbError(f"an in-loop homotopy schedule is implemented for PTR only, not for {algo}")
         self.scale = SCPScaling(traj, handle, self.t)
         self._build()
 
@@ -417,6 +419,10 @@ class SCPBatchSolution:      # batched SCPSolution (scp.jl:105-119)
     raw_status: np.ndarray
     tc: np.ndarray = None       # continuous-time grid and state trajectory xc (B, res, nx): filled by propagate()
     xc: np.ndarray = None
+    hom_index: np.ndarray = None    # in-loop homotopy schedule: final grid index per seed (B,),
+    iter_max: np.ndarray = None     # effective iter_max per seed (B,; without a schedule the configured one),
+    hom_history: dict = None        # {"index", "improv_rel"} (B, cap): per iteration the grid index the subproblem was
+                                    # built with and its improv_rel (-1 / NaN after the seed's last iteration)
 
 
 def create(pars: Parameters, traj, handle, l1_block=4) -> SCPProblem:
@@ -431,11 +437,38 @@ def set_parameters(pbm: SCPProblem, par=None):
     pbm.handle._check(pbm.handle.lib.scpb_ptr_set_par(pbm.ptr, pp, par.size), "scpb_ptr_set_par")
 
 
-def solve(pbm: SCPProblem, guesses=None, **cone_opts) -> SCPBatchSolution:
+def homotopy_history_length(pbm: SCPProblem):
+    """the most iterations a seed can run under the problem's schedule: every update extends its iter_max by the
+    iterations since the previous one, so iter_max + (n_grid - 1)(iter_max - 1)"""
+    n, it = pbm.traj.hom["grid"].size, pbm.pars.iter_max
+    return it + (n - 1) * max(it - 1, 0)
+
+
+def set_homotopy(pbm: SCPProblem, B, beta=None):
+    """Push the problem's in-loop homotopy schedule (problem_set_homotopy_update) and the per-seed thresholds of the next
+    solve to the device (scpb_ptr_set_homotopy, scpb_ptr_set_homotopy_beta); a problem without one detaches it."""
+    h, hom = pbm.handle, getattr(pbm.traj, "hom", None)
+    if hom is None:
+        if beta is not None:
+            raise lib.ScpbError("beta is the update threshold of a homotopy schedule, and the problem has none "
+                                "(problem_set_homotopy_update)")
+        h._check(h.lib.scpb_ptr_set_homotopy(pbm.ptr, 0, 0, None, 0.0), "scpb_ptr_set_homotopy")
+        return
+    slot = -1 if hom["par_index"] is None else hom["par_index"]        # -1: the slot the pack reads its parameter from
+    grid, pg = lib._f64(hom["grid"])
+    h._check(h.lib.scpb_ptr_set_homotopy(pbm.ptr, int(slot), grid.size, pg, hom["worsen_tol"]), "scpb_ptr_set_homotopy")
+    b = np.ascontiguousarray(np.broadcast_to(np.asarray(hom["beta"] if beta is None else beta, dtype=np.float64), (B,)))
+    b, pb = lib._f64(b)
+    h._check(h.lib.scpb_ptr_set_homotopy_beta(pbm.ptr, B, pb), "scpb_ptr_set_homotopy_beta")
+
+
+def solve(pbm: SCPProblem, guesses=None, beta=None, **cone_opts) -> SCPBatchSolution:
     """PTR.solve (ptr.jl:448-532) for a batch: guesses = (xd0 (B,N,nx), ud0 (B,N,nu), p0 (B,np));
     None => the problem's own guess (one seed).  The model's parameter block is read again here, as the reference's
     closures read the model at call time: a parameter changed between two solves (a homotopy step) takes effect
-    without a new create."""
+    without a new create.
+    beta: update threshold of the problem's in-loop homotopy schedule, a scalar or one per seed (None: the one given to
+    problem_set_homotopy_update), so a sweep over thresholds is one batch."""
     traj, pars, h = pbm.traj, pbm.pars, pbm.handle
     set_parameters(pbm)
     if guesses is None:
@@ -448,6 +481,7 @@ def solve(pbm: SCPProblem, guesses=None, **cone_opts) -> SCPBatchSolution:
     p0 = np.ascontiguousarray(guesses[2], dtype=np.float64)
     B, N = xd0.shape[0], pars.N
     assert xd0.shape == (B, N, traj.nx) and ud0.shape == (B, N, traj.nu) and p0.shape == (B, traj.np)
+    set_homotopy(pbm, B, beta)
     o = lib.ConeOpts()
     o.nref = -1
     o.equil = -1
@@ -472,7 +506,16 @@ def solve(pbm: SCPProblem, guesses=None, **cone_opts) -> SCPBatchSolution:
     tm = dict(discretize=timing[0], formulate=timing[1], solve=timing[2], overhead=timing[3], total=timing[4],
               lockstep_iterations=int(timing[5]), ipm_iterations=int(timing[6]), chunks=int(timing[7]),
               initial_discretize=timing[8])
-    return SCPBatchSolution(names, iters, J, pbm.t, xd, ud, p, dev, feas, tm, status)
+    sol = SCPBatchSolution(names, iters, J, pbm.t, xd, ud, p, dev, feas, tm, status)
+    sol.iter_max = np.full(B, pars.iter_max, dtype=np.int32)
+    if getattr(traj, "hom", None) is not None:
+        cap = homotopy_history_length(pbm)
+        sol.hom_index = np.zeros(B, dtype=np.int32)
+        hidx, himp = np.zeros((B, cap), dtype=np.int32), np.zeros((B, cap))
+        rc = h.lib.scpb_ptr_homotopy_result(pbm.ptr, B, ip(sol.hom_index), ip(sol.iter_max), cap, ip(hidx), dp(himp))
+        h._check(rc, "scpb_ptr_homotopy_result")
+        sol.hom_history = {"index": hidx, "improv_rel": himp}
+    return sol
 
 
 def correct_convex(pbm: SCPProblem, guesses, **cone_opts):
