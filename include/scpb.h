@@ -225,10 +225,10 @@ int32_t scpb_ptr_homotopy_result(scpb_ptr s, int32_t B, int32_t *hom_index, int3
  * 2+16*cone_status = SCP_FAILED), iteration counts, J_aug, deviation, dynamic feasibility flags and
  * timing[10] = {discretize, formulate, solve, overhead, total seconds, longest PTR chain (iterations),
  * interior-point iterations summed over seeds and subproblems, number of seed chunks, seconds of the initial
- * full-batch discretize!, 0}.  The batch is cut into chunks of whole seed groups and every chunk runs its own sequence of
- * PTR iterations on its own CUDA stream (seeds are independent; SCPB_PTR_CHUNKS=<n> sets the number of chunks, default 64,
- * 0 or 1 = one lock-step loop over the whole batch): the four phase times are then those of chunk 0's chain, the total is
- * the whole call. */
+ * full-batch discretize!, 0}.  By default (SCPB_PTR_CHUNKS unset, 0 or 1) one lock-step loop runs over the whole batch.
+ * SCPB_PTR_CHUNKS=<n> cuts the batch into n chunks of whole seed groups and every chunk runs its own sequence of PTR
+ * iterations on its own CUDA stream (seeds are independent): the four phase times are then those of chunk 0's chain,
+ * the total is the whole call. */
 int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *ud0, const double *p0,
                        const scpb_cone_opts *opts, double *xd, double *ud, double *p, int32_t *status,
                        int32_t *iters, double *J, double *deviation, int32_t *feas, double *timing);
@@ -240,9 +240,10 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
  * rows Q (over the scaled solver variables of the x, u, p blocks, constants Q_const) of
  *   row 0: original cost L(x,u,p);  rows 1..n_ic: g_ic(x_1,p);  rows n_ic+1..n_ic+n_tc: g_tc(x_N,p)
  * which, with the defects of discretize! and the constraint pack's s, give the nonlinear augmented cost
- * (actual_cost_penalty!, scvx.jl:919-951).  scpb_scvx_solve returns what SCPSolution keeps of the last subproblem
- * (scp.jl:205-236): trajectory, status (0/1 solved, 2+16*cone status failed), iterations, J_aug, deviation, feas,
- * and the final trust-region radius per seed. */
+ * (actual_cost_penalty!, scvx.jl:919-951).  That cost has the penalty of the starship's constraint pack only:
+ * scpb_scvx_attach refuses a problem with another pack (SCPB_ERR_UNSUPPORTED).  scpb_scvx_solve returns what
+ * SCPSolution keeps of the last subproblem (scp.jl:205-236): trajectory, status (0/1 solved, 2+16*cone status failed),
+ * iterations, J_aug, deviation, feas, and the final trust-region radius per seed. */
 typedef struct {
     double lam, rho_0, rho_1, rho_2, beta_sh, beta_gr, eta_init, eta_lb, eta_ub;
     int32_t oeta, n_ic, n_tc, reserved;

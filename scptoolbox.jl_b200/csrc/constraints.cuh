@@ -22,6 +22,17 @@ struct HomSlot { static constexpr int value = -1; };
 template <class CP>
 struct HomSlot<CP, std::void_t<decltype(CP::KAPPA)>> { static constexpr int value = CP::KAPPA; };
 
+// the constraint pack of model ID; Constr<0> (no constraints) for a model without one
+template <int ID>
+using PackOf = std::conditional_t<(Constr<ID>::NS > 0), Constr<ID>, Constr<0>>;
+
+// calls f(PackOf<id>()) when has_pack, f(Constr<0>()) otherwise or for an unknown id
+template <class F>
+void with_constr(int id, bool has_pack, F &&f)
+{
+    if (!has_pack || !with_model(id, [&](auto m) { f(PackOf<ModelId<decltype(m)>::value>()); })) f(Constr<0>());
+}
+
 // the pack at node k; a pack with a homotopy parameter takes it from *kap (a seed's own value) unless kap is null
 template <class CP>
 __device__ __forceinline__ void constr_eval(const ModelPar &P, const double *kap, double t, int N, int k, const double *x,

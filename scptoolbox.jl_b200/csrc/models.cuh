@@ -357,3 +357,25 @@ struct Model<SCPB_MODEL_RENDEZVOUS2D> {
     }
     __device__ __forceinline__ static void post_step(double *) {}
 };
+
+// ---------------------------------------------------------------- host dispatch on the model id
+template <class M>
+struct ModelId;
+template <int ID>
+struct ModelId<Model<ID>> { static constexpr int value = ID; };
+
+// calls f(Model<id>()) and returns true; false for an id without a pack.  Every per-model switch goes through here,
+// so a new model is one more case.
+template <class F>
+bool with_model(int id, F &&f)
+{
+    switch (id) {
+    case SCPB_MODEL_DBLINT: f(Model<SCPB_MODEL_DBLINT>()); return true;
+    case SCPB_MODEL_ROCKET: f(Model<SCPB_MODEL_ROCKET>()); return true;
+    case SCPB_MODEL_STARSHIP: f(Model<SCPB_MODEL_STARSHIP>()); return true;
+    case SCPB_MODEL_QUADROTOR: f(Model<SCPB_MODEL_QUADROTOR>()); return true;
+    case SCPB_MODEL_FREEFLYER: f(Model<SCPB_MODEL_FREEFLYER>()); return true;
+    case SCPB_MODEL_RENDEZVOUS2D: f(Model<SCPB_MODEL_RENDEZVOUS2D>()); return true;
+    default: return false;
+    }
+}

@@ -11,6 +11,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdio>
+#include <functional>
 #include <thread>
 #include "handle.cuh"
 #include "discretize.cuh"
@@ -173,25 +174,17 @@ __device__ __forceinline__ double qnorm_acc(double acc, double v, int q)
     return q == 0 ? fmax(acc, v) : (q == 1 ? acc + v : acc + v * v);
 }
 
-// one thread per seed: deviation, predicted improvement, stopping rule, acceptance (ptr.jl:908-932, 509)
-__global__ void k_ptr_step(const StepDev d)
+// The per-seed helpers below are shared by the step kernels of PTR (StepDev), SCvx (ScvxDev) and GuSTO (GustoDev):
+// each reads the fields of the same name that all three descriptors carry.
+
+// solution_deviation (scp.jl:909-931) of seed b's candidate (xn, and pn: its parameter block) from its reference (xd,
+// p), in scaled units
+template <class D>
+__device__ __forceinline__ double solution_deviation(const D &d, int b, const double *pn)
 {
-    const int q_ = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q_ >= (d.nb > 0 ? d.nb : d.B)) return;
-    const int b = d.b0 + q_;
-    if (b >= d.B) return;
-    if (d.done[b]) return;
-    if (d.ipm_total) atomicAdd(d.ipm_total, (unsigned long long)d.cone_iters[b]);
-    const int cs = d.cone_status[b];
-    if (d.hom_n > 0) d.hist_idx[(size_t)b * d.hist_cap + d.iter - 1] = d.hom_idx[b];
-    if (!(cs == IPM_OPTIMAL || cs == IPM_ALMOST)) {  // unsafe_solution, scp.jl:965-980: before the callback (ptr.jl:488-491)
-        d.done[b] = 1; d.status[b] = 2 + 16 * cs; d.iters[b] = d.iter;
-        if (d.ndone) atomicAdd(d.ndone, 1);
-        return;
-    }
     const int q = d.q_exit;
     double dp = 0.0;
-    for (int j = 0; j < d.np; j++) dp = qnorm_acc(dp, (d.pn[(size_t)b * d.np + j] - d.p[(size_t)b * d.np + j]) / d.Sp[j], q);
+    for (int j = 0; j < d.np; j++) dp = qnorm_acc(dp, (pn[j] - d.p[(size_t)b * d.np + j]) / d.Sp[j], q);
     if (q == 2) dp = sqrt(dp);
     double dx = 0.0;
     for (int k = 0; k < d.N; k++) {
@@ -203,7 +196,54 @@ __global__ void k_ptr_step(const StepDev d)
         if (q == 2) a = sqrt(a);
         dx = fmax(dx, a);
     }
-    const double deviation = dp + dx;
+    return dp + dx;
+}
+
+// unsafe_solution (scp.jl:965-980): a seed whose subproblem is not (almost) optimal stops with status 2 + 16 * cone status
+template <class D>
+__device__ __forceinline__ bool unsafe_exit(const D &d, int b, int cs, int *ndone)
+{
+    if (cs == IPM_OPTIMAL || cs == IPM_ALMOST) return false;
+    d.done[b] = 1; d.status[b] = 2 + 16 * cs; d.iters[b] = d.iter;
+    if (ndone) atomicAdd(ndone, 1);
+    return true;
+}
+
+// the candidate becomes seed b's reference, with cost J
+template <class D>
+__device__ __forceinline__ void accept_candidate(const D &d, int b, double J)
+{
+    for (int k = 0; k < d.N; k++) {
+        for (int j = 0; j < d.nx; j++) { const size_t o = ((size_t)b * d.N + k) * d.nx + j; d.xd[o] = d.xn[o]; }
+        for (int j = 0; j < d.nu; j++) { const size_t o = ((size_t)b * d.N + k) * d.nu + j; d.ud[o] = d.un[o]; }
+    }
+    for (int j = 0; j < d.np; j++) d.p[(size_t)b * d.np + j] = d.pn[(size_t)b * d.np + j];
+    d.J_ref[b] = J;
+}
+
+// value of solver variable v (scaled) at the physical trajectory (x, u, p): only x, u, p blocks may appear
+template <class D>
+__device__ __forceinline__ double scaled_var(const D &d, const double *x, const double *u, const double *p, int v)
+{
+    if (v >= d.vx && v < d.vx + d.N * d.nx) { const int e = v - d.vx, i = e % d.nx; return (x[e] - d.cx[i]) / d.Sx[i]; }
+    if (v >= d.vu && v < d.vu + d.N * d.nu) { const int e = v - d.vu, i = e % d.nu; return (u[e] - d.cu[i]) / d.Su[i]; }
+    const int j = v - d.vp;
+    return (p[j] - d.cp[j]) / d.Sp[j];
+}
+
+// one thread per seed: deviation, predicted improvement, stopping rule, acceptance (ptr.jl:908-932, 509)
+__global__ void k_ptr_step(const StepDev d)
+{
+    const int q_ = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q_ >= (d.nb > 0 ? d.nb : d.B)) return;
+    const int b = d.b0 + q_;
+    if (b >= d.B) return;
+    if (d.done[b]) return;
+    if (d.ipm_total) atomicAdd(d.ipm_total, (unsigned long long)d.cone_iters[b]);
+    const int cs = d.cone_status[b];
+    if (d.hom_n > 0) d.hist_idx[(size_t)b * d.hist_cap + d.iter - 1] = d.hom_idx[b];
+    if (unsafe_exit(d, b, cs, d.ndone)) return;   // before the callback (ptr.jl:488-491)
+    const double deviation = solution_deviation(d, b, d.pn + (size_t)b * d.np);
     const double Jr = d.J_ref[b], Jn = d.J_new[b];
     const double imp = (Jr - Jn) / fabs(Jr);
     d.dev[b] = deviation; d.imp[b] = imp;
@@ -223,13 +263,7 @@ __global__ void k_ptr_step(const StepDev d)
             d.hom_last[b] = d.iter;
         }
     }
-    // accept: ref <- sol
-    for (int k = 0; k < d.N; k++) {
-        for (int j = 0; j < d.nx; j++) { const size_t o = ((size_t)b * d.N + k) * d.nx + j; d.xd[o] = d.xn[o]; }
-        for (int j = 0; j < d.nu; j++) { const size_t o = ((size_t)b * d.N + k) * d.nu + j; d.ud[o] = d.un[o]; }
-    }
-    for (int j = 0; j < d.np; j++) d.p[(size_t)b * d.np + j] = d.pn[(size_t)b * d.np + j];
-    d.J_ref[b] = Jn;
+    accept_candidate(d, b, Jn);
     d.iters[b] = d.iter;
     if (stop && !acted) {
         d.done[b] = 1; d.status[b] = 0;
@@ -468,7 +502,7 @@ static int run_discretize(scpb_ptr_s *s, int B, int G, const double *xd, const d
 // ----------------------------------------------------------------------------------------------
 // SCvx (src/solvers/scvx.jl): nonlinear augmented cost, ratio test, accept / reject, radius update
 struct ScvxDev {
-    int B, G, N, nx, nu, np, n_ic, n_tc, vx, vu, vp, q_exit, iter, iter_max, nsrc, dltv_lo, dltv_hi;
+    int N, nx, nu, np, n_ic, n_tc, vx, vu, vp, q_exit, iter, iter_max, B;
     double lam, rho_0, rho_1, rho_2, beta_sh, beta_gr, eta_lb, eta_ub, eps_abs, eps_rel;
     const int *Q_rp, *Q_ci;
     const double *Q_v, *Q_c;
@@ -478,17 +512,11 @@ struct ScvxDev {
     double *J_ref, *J_new, *L_new, *J_out, *eta, *dev;
     const int *cone_status, *feas_new;
     int *done, *status, *iters, *nactive, *accept;
-    double *src, *src2;
 };
 
-// value of solver variable v (scaled) at the physical trajectory (x, u, p): only x, u, p blocks may appear in Q
-__device__ __forceinline__ double scvx_var(const ScvxDev &d, const double *x, const double *u, const double *p, int v)
-{
-    if (v >= d.vx && v < d.vx + d.N * d.nx) { const int e = v - d.vx, i = e % d.nx; return (x[e] - d.cx[i]) / d.Sx[i]; }
-    if (v >= d.vu && v < d.vu + d.N * d.nu) { const int e = v - d.vu, i = e % d.nu; return (u[e] - d.cu[i]) / d.Su[i]; }
-    const int j = v - d.vp;
-    return (p[j] - d.cp[j]) / d.Sp[j];
-}
+// the constraint packs k_scvx_cost has the penalty of (none, the starship's): scpb_scvx_attach refuses any other
+template <class CP>
+constexpr bool scvx_has_pack = CP::NS == 0 || std::is_same_v<CP, Constr<SCPB_MODEL_STARSHIP>>;
 
 // one thread per seed: J = L + lambda (trapz_k(|defect_k|_1 + |max(s_k, 0)|_1) + |g_ic|_1 + |g_tc|_1)
 // (solution_cost! / actual_cost_penalty!, scvx.jl:919-988) of the trajectory (x, u, p) whose defects are in d.defect
@@ -502,7 +530,7 @@ __global__ void k_scvx_cost(const ScvxDev d, const double *xall, const double *u
     double q0 = 0.0, gsum = 0.0;
     for (int r = 0; r < 1 + d.n_ic + d.n_tc; r++) {
         double acc = d.Q_c[r];
-        for (int k = d.Q_rp[r]; k < d.Q_rp[r + 1]; k++) acc = fma(d.Q_v[k], scvx_var(d, x, u, p, d.Q_ci[k]), acc);
+        for (int k = d.Q_rp[r]; k < d.Q_rp[r + 1]; k++) acc = fma(d.Q_v[k], scaled_var(d, x, u, p, d.Q_ci[k]), acc);
         if (r == 0) q0 = acc; else gsum += fabs(acc);
     }
     double pen = 0.0, Pprev = 0.0;
@@ -533,26 +561,8 @@ __global__ void k_scvx_step(const ScvxDev d)
     if (b >= d.B) return;
     d.accept[b] = 0;
     if (d.done[b]) return;
-    const int cs = d.cone_status[b];
-    if (!(cs == IPM_OPTIMAL || cs == IPM_ALMOST)) {  // unsafe_solution, scp.jl:965-980
-        d.done[b] = 1; d.status[b] = 2 + 16 * cs; d.iters[b] = d.iter;
-        return;
-    }
-    const int q = d.q_exit;
-    double dp = 0.0;
-    for (int j = 0; j < d.np; j++) dp = qnorm_acc(dp, (d.pn[(size_t)b * d.np + j] - d.p[(size_t)b * d.np + j]) / d.Sp[j], q);
-    if (q == 2) dp = sqrt(dp);
-    double dx = 0.0;
-    for (int k = 0; k < d.N; k++) {
-        double a = 0.0;
-        for (int j = 0; j < d.nx; j++) {
-            const size_t o = ((size_t)b * d.N + k) * d.nx + j;
-            a = qnorm_acc(a, (d.xn[o] - d.xd[o]) / d.Sx[j], q);
-        }
-        if (q == 2) a = sqrt(a);
-        dx = fmax(dx, a);
-    }
-    const double deviation = dp + dx;
+    if (unsafe_exit(d, b, d.cone_status[b], nullptr)) return;
+    const double deviation = solution_deviation(d, b, d.pn + (size_t)b * d.np);
     d.dev[b] = deviation;
     const double Jr = d.J_ref[b], Jn = d.J_new[b], Ln = d.L_new[b];
     const double pre = Jr - Ln;                        // pre_improv = J_ref - L(sol)  (scvx.jl:724-726)
@@ -569,14 +579,7 @@ __global__ void k_scvx_step(const ScvxDev d)
         d.eta[b] = eta;
     }
     const bool last = stop || d.iter >= d.iter_max;
-    if (acc || last) {
-        for (int k = 0; k < d.N; k++) {
-            for (int j = 0; j < d.nx; j++) { const size_t o = ((size_t)b * d.N + k) * d.nx + j; d.xd[o] = d.xn[o]; }
-            for (int j = 0; j < d.nu; j++) { const size_t o = ((size_t)b * d.N + k) * d.nu + j; d.ud[o] = d.un[o]; }
-        }
-        for (int j = 0; j < d.np; j++) d.p[(size_t)b * d.np + j] = d.pn[(size_t)b * d.np + j];
-        d.J_ref[b] = Jn;
-    }
+    if (acc || last) accept_candidate(d, b, Jn);
     d.accept[b] = (acc && !last) ? 1 : 0;
     d.J_out[b] = Jn;
     d.iters[b] = d.iter;
@@ -584,17 +587,18 @@ __global__ void k_scvx_step(const ScvxDev d)
     else atomicAdd(d.nactive, 1);
 }
 
-// accepted seeds: the candidate's DLTV blocks (written by discretize! into src2) become the reference linearisation
-__global__ void k_scvx_take_dltv(const ScvxDev d)
+// SCvx and GuSTO, accepted seeds: the candidate's DLTV blocks [lo, hi) (written by discretize! into src2) become the
+// reference linearisation in src
+__global__ void k_scvx_take_dltv(int B, int G, int nsrc, int lo, int hi, const int *accept, double *src, const double *src2)
 {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long span = d.dltv_hi - d.dltv_lo;
-    if (i >= span * d.B) return;
-    const int b = (int)(i % d.B);
-    if (!d.accept[b]) return;
-    const long long e = d.dltv_lo + i / d.B;
-    const size_t a = gaddr(b, d.G, d.nsrc, e);
-    d.src[a] = d.src2[a];
+    const long long span = hi - lo;
+    if (i >= span * B) return;
+    const int b = (int)(i % B);
+    if (!accept[b]) return;
+    const long long e = lo + i / B;
+    const size_t a = gaddr(b, G, nsrc, e);
+    src[a] = src2[a];
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -664,15 +668,6 @@ __global__ void k_gusto_nodes(const GustoDev d)
     d.nodef[i] = viol;
 }
 
-// value of solver variable v (scaled) at the physical trajectory (x, u, p)
-__device__ __forceinline__ double gusto_var(const GustoDev &d, const double *x, const double *u, const double *p, int v)
-{
-    if (v >= d.vx && v < d.vx + d.N * d.nx) { const int e = v - d.vx, i = e % d.nx; return (x[e] - d.cx[i]) / d.Sx[i]; }
-    if (v >= d.vu && v < d.vu + d.N * d.nu) { const int e = v - d.vu, i = e % d.nu; return (u[e] - d.cu[i]) / d.Su[i]; }
-    const int j = v - d.vp;
-    return (p[j] - d.cp[j]) / d.Sp[j];
-}
-
 // one thread per seed: SubproblemSolution(spbm) costs (gusto.jl:399-418), check_stopping_criterion! (:1203-1231),
 // update_trust_region! (:1245-1293) and update_rule! (:1310-1427, with the mu-shrink of the next subproblem's eta, :268).
 __global__ void k_gusto_step(const GustoDev d)
@@ -681,17 +676,13 @@ __global__ void k_gusto_step(const GustoDev d)
     if (b >= d.B) return;
     d.accept[b] = 0;
     if (d.done[b]) return;
-    const int cs = d.cone_status[b];
-    if (!(cs == IPM_OPTIMAL || cs == IPM_ALMOST)) {  // unsafe_solution, scp.jl:965-980
-        d.done[b] = 1; d.status[b] = 2 + 16 * cs; d.iters[b] = d.iter;
-        return;
-    }
+    if (unsafe_exit(d, b, d.cone_status[b], nullptr)) return;
     const double *x = d.xn + (size_t)b * d.N * d.nx, *u = d.un + (size_t)b * d.N * d.nu, *p = d.pn + (size_t)b * d.np;
     // original cost J of the candidate: affine row + weighted squares (original_cost, gusto.jl:680-707)
     double J = 0.0;
     for (int r = 0; r <= d.nsq; r++) {
         double acc = d.Q_c[r];
-        for (int k = d.Q_rp[r]; k < d.Q_rp[r + 1]; k++) acc = fma(d.Q_v[k], gusto_var(d, x, u, p, d.Q_ci[k]), acc);
+        for (int k = d.Q_rp[r]; k < d.Q_rp[r + 1]; k++) acc = fma(d.Q_v[k], scaled_var(d, x, u, p, d.Q_ci[k]), acc);
         J += r == 0 ? acc : d.Q_w[r - 1] * acc * acc;
     }
     // soft trust-region cost as the subproblem measured it (J_tr = value(L_tr), gusto.jl:409); the row is L_tr / lambda
@@ -718,22 +709,7 @@ __global__ void k_gusto_step(const GustoDev d)
     const double eta = d.eta[b], lam = d.lam[b];
     J_tr *= lam;
     const double J_aug = J + J_st + J_tr, L_aug = d.L_aug[b];
-    // deviation from the reference (solution_deviation, scp.jl:909-931)
-    const int q = d.q_exit;
-    double dp = 0.0;
-    for (int j = 0; j < d.np; j++) dp = qnorm_acc(dp, (p[j] - d.p[(size_t)b * d.np + j]) / d.Sp[j], q);
-    if (q == 2) dp = sqrt(dp);
-    double dx = 0.0;
-    for (int k = 0; k < d.N; k++) {
-        double a = 0.0;
-        for (int j = 0; j < d.nx; j++) {
-            const size_t o = ((size_t)b * d.N + k) * d.nx + j;
-            a = qnorm_acc(a, (d.xn[o] - d.xd[o]) / d.Sx[j], q);
-        }
-        if (q == 2) a = sqrt(a);
-        dx = fmax(dx, a);
-    }
-    const double deviation = dp + dx;
+    const double deviation = solution_deviation(d, b, p);
     d.dev[b] = deviation;
     const double Jr = d.J_ref[b];
     const double dJ = fabs(Jr - J_aug) / fabs(Jr);
@@ -756,14 +732,7 @@ __global__ void k_gusto_step(const GustoDev d)
         d.eta[b] = n_eta; d.lam[b] = n_lam;
     }
     const bool last = stop || d.iter >= d.iter_max;
-    if (acc || last) {   // the candidate becomes the reference; it is also what the loop returns when it ends (scp.jl:205-236)
-        for (int k = 0; k < d.N; k++) {
-            for (int j = 0; j < d.nx; j++) { const size_t o = ((size_t)b * d.N + k) * d.nx + j; d.xd[o] = d.xn[o]; }
-            for (int j = 0; j < d.nu; j++) { const size_t o = ((size_t)b * d.N + k) * d.nu + j; d.ud[o] = d.un[o]; }
-        }
-        for (int j = 0; j < d.np; j++) d.p[(size_t)b * d.np + j] = d.pn[(size_t)b * d.np + j];
-        d.J_ref[b] = J_aug;
-    }
+    if (acc || last) accept_candidate(d, b, J_aug);   // also what the loop returns when it ends (scp.jl:205-236)
     d.accept[b] = (acc && !last) ? 1 : 0;
     d.J_out[b] = J_aug;            // SCPSolution.cost = last_sol.J_aug (scp.jl:236)
     d.iters[b] = d.iter;
@@ -780,13 +749,8 @@ __global__ void k_fill(double *v, double a, int n)
 // nonconvex-constraint linearisation with the pack of the problem's model (none: only the scaled references)
 static void launch_linearize(scpb_ptr_s *s, const PtrDev &pd, int nbn, cudaStream_t st)
 {
-    const bool has = s->d.ns > 0;
-    if (has && s->model_id == SCPB_MODEL_STARSHIP) k_linearize<Constr<SCPB_MODEL_STARSHIP>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-    else if (has && s->model_id == SCPB_MODEL_FREEFLYER) k_linearize<Constr<SCPB_MODEL_FREEFLYER>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-    else if (has && s->model_id == SCPB_MODEL_QUADROTOR) k_linearize<Constr<SCPB_MODEL_QUADROTOR>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-    else if (has && s->model_id == SCPB_MODEL_RENDEZVOUS2D)
-        k_linearize<Constr<SCPB_MODEL_RENDEZVOUS2D>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-    else k_linearize<Constr<0>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
+    with_constr(s->model_id, s->d.ns > 0,
+                [&](auto cp) { k_linearize<decltype(cp)><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p); });
 }
 
 // scpb_debug_constraints: the pack's s, C, D, G at every (seed, node), one thread each
@@ -836,34 +800,229 @@ static int debug_constr_t(scpb_handle_s *h, int B, int N, int ns, int ng, const 
     return rc;
 }
 
-template <class M, class CP>
-static void launch_gusto_nodes_t(const GustoDev &gd, int nbn, cudaStream_t st)
-{
-    k_gusto_nodes<M, CP><<<nbn, 64, 0, st>>>(gd);
-}
-
+// GuSTO's node terms with the problem's model and pack; SCPB_ERR_UNSUPPORTED for the rendezvous, which GuSTO lacks
 static int launch_gusto_nodes(scpb_ptr_s *s, const GustoDev &gd, cudaStream_t st)
 {
     const int nbn = (int)(((long long)gd.B * gd.N + 63) / 64);
-    const bool has = s->d.ns > 0;
-    switch (s->model_id) {
-    case SCPB_MODEL_DBLINT: launch_gusto_nodes_t<Model<SCPB_MODEL_DBLINT>, Constr<0>>(gd, nbn, st); break;
-    case SCPB_MODEL_ROCKET: launch_gusto_nodes_t<Model<SCPB_MODEL_ROCKET>, Constr<0>>(gd, nbn, st); break;
-    case SCPB_MODEL_STARSHIP:
-        if (has) launch_gusto_nodes_t<Model<SCPB_MODEL_STARSHIP>, Constr<SCPB_MODEL_STARSHIP>>(gd, nbn, st);
-        else launch_gusto_nodes_t<Model<SCPB_MODEL_STARSHIP>, Constr<0>>(gd, nbn, st);
-        break;
-    case SCPB_MODEL_QUADROTOR:
-        if (has) launch_gusto_nodes_t<Model<SCPB_MODEL_QUADROTOR>, Constr<SCPB_MODEL_QUADROTOR>>(gd, nbn, st);
-        else launch_gusto_nodes_t<Model<SCPB_MODEL_QUADROTOR>, Constr<0>>(gd, nbn, st);
-        break;
-    case SCPB_MODEL_FREEFLYER:
-        if (has) launch_gusto_nodes_t<Model<SCPB_MODEL_FREEFLYER>, Constr<SCPB_MODEL_FREEFLYER>>(gd, nbn, st);
-        else launch_gusto_nodes_t<Model<SCPB_MODEL_FREEFLYER>, Constr<0>>(gd, nbn, st);
-        break;
-    default: return SCPB_ERR_UNSUPPORTED;
+    int rc = SCPB_ERR_UNSUPPORTED;
+    with_model(s->model_id, [&](auto m) {
+        using M = decltype(m);
+        constexpr int id = ModelId<M>::value;
+        if constexpr (id != SCPB_MODEL_RENDEZVOUS2D) {
+            if (s->d.ns > 0) k_gusto_nodes<M, PackOf<id>><<<nbn, 64, 0, st>>>(gd);
+            else k_gusto_nodes<M, Constr<0>><<<nbn, 64, 0, st>>>(gd);
+            rc = SCPB_OK;
+        }
+    });
+    return rc;
+}
+
+// ----------------------------------------------------------------------------------------------
+// One solve of PTR, SCvx or GuSTO: the state that solve_begin sets up, the loop body each algorithm parameterises, and
+// the outputs solve_end returns.
+struct Solve {
+    scpb_ptr_s *s;
+    scpb_handle_s *h;
+    cudaStream_t st;
+    int B, G;
+    IpmData *D;
+    IpmOpts o;
+    PtrDev pd{};
+    AsmDev ad{};
+    StepDev sd{};
+    // the algorithm: cone options of iteration it, where discretize! writes the candidate's DLTV (nullptr: src), the
+    // candidate's cost (run in the discretize phase; may be empty) and the step that accepts, rejects and stops
+    std::function<IpmOpts(int)> opts_at;
+    double *cand_src = nullptr;
+    std::function<int()> candidate;
+    std::function<int(int it, cudaStream_t st, int nb)> step;
+    // phase timers (the reference's keys: discretize / formulate / solve / overhead, scp.jl:177-178,990-995): phase id
+    // of the interval that ENDS at event i
+    EventList evl;
+    std::vector<int> phase;
+    int total_it = 0, n_chunks = 0;
+    long long ipm_iters = 0;
+    std::vector<int> init_status;   // sources of the resets' uploads, kept until the solve ends
+    std::vector<double> nanv;
+    void mark(int ph, cudaStream_t on)
+    {
+        cudaEvent_t e;
+        cudaEventCreate(&e); cudaEventRecord(e, on);
+        evl.ev.push_back(e); phase.push_back(ph);
+    }
+};
+
+// what every solve does before its loop: check the batch, select the model, pick the seed group size G, reserve the
+// buffers, upload the guesses, reset the per-seed state and describe it to the kernels
+static int solve_begin(Solve &v, scpb_ptr_s *s, int B, const double *xd0, const double *ud0, const double *p0,
+                       const scpb_cone_opts *opts, const char *who)
+{
+    scpb_handle_s *h = s->h;
+    if (B <= 0 || !xd0 || !ud0 || !p0) return set_err(h, SCPB_ERR_ARG, "%s: bad arguments", who);
+    SCPB_CUDA(h, cudaSetDevice(h->device));
+    ptr_select_model(s);
+    SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
+    const scpb_ptr_desc &d = s->d;
+    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
+    int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
+    if (rc) return rc;
+    if ((rc = ptr_reserve(s, B, G))) return rc;
+    if (s->hom_n > 0) {   // PTR only: SCvx and GuSTO refuse a problem with a schedule
+        if ((int)s->hom_beta_h.size() != B)
+            return set_err(h, SCPB_ERR_STATE, "%s: the homotopy schedule has %d update thresholds for %d seeds "
+                           "(scpb_ptr_set_homotopy_beta)", who, (int)s->hom_beta_h.size(), B);
+        if ((rc = hom_reserve(s, s->capB))) return rc;
+    }
+    IpmData *D = scpb_internal_cone_data(s->cone);
+    const ConeSymbolic *S = scpb_internal_cone_sym(s->cone);
+    v.s = s; v.h = h; v.st = h->stream; v.B = B; v.G = G; v.D = D;
+    v.o = scpb_internal_make_opts(opts);
+    cudaStream_t st = h->stream;
+    SCPB_CUDA(h, cudaMemcpyAsync(s->xd, xd0, sizeof(double) * B * d.N * d.nx, cudaMemcpyHostToDevice, st));
+    SCPB_CUDA(h, cudaMemcpyAsync(s->ud, ud0, sizeof(double) * B * d.N * d.nu, cudaMemcpyHostToDevice, st));
+    SCPB_CUDA(h, cudaMemcpyAsync(s->p, p0, sizeof(double) * B * d.np, cudaMemcpyHostToDevice, st));
+    SCPB_CUDA(h, cudaMemsetAsync(s->src, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
+    if (s->src2) SCPB_CUDA(h, cudaMemsetAsync(s->src2, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
+    SCPB_CUDA(h, cudaMemsetAsync(s->done, 0, sizeof(int) * s->capB, st));
+    SCPB_CUDA(h, cudaMemsetAsync(s->iters, 0, sizeof(int) * s->capB, st));
+    v.init_status.assign(s->capB, 1);
+    SCPB_CUDA(h, cudaMemcpyAsync(s->status, v.init_status.data(), sizeof(int) * s->capB, cudaMemcpyHostToDevice, st));
+    v.nanv.assign(s->capB, nan(""));
+    SCPB_CUDA(h, cudaMemcpyAsync(s->devi, v.nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
+    if (s->J_out) SCPB_CUDA(h, cudaMemcpyAsync(s->J_out, v.nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
+    // PTR and GuSTO start from J_ref = NaN (the guess has no cost); SCvx overwrites it with the guess's cost
+    SCPB_CUDA(h, cudaMemcpyAsync(s->J_ref, v.nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
+
+    const size_t nsc = (size_t)(d.nx + d.nu + d.np);
+    const double *Sx = s->scale, *Su = Sx + d.nx, *Sp = Su + d.nu, *cx = s->scale + nsc, *cu = cx + d.nx, *cp = cu + d.nu;
+    PtrDev &pd = v.pd;
+    pd.B = B; pd.G = G; pd.N = d.N; pd.nx = d.nx; pd.nu = d.nu; pd.np = d.np; pd.ns = d.ns;
+    pd.nsrc = d.nsrc; pd.oC = d.oC; pd.oD = d.oD; pd.oG = d.oG; pd.ors = d.ors; pd.oxh = d.oxh; pd.ouh = d.ouh; pd.oph = d.oph;
+    pd.t_grid = s->tgrid; pd.Sx = Sx; pd.cx = cx; pd.Su = Su; pd.cu = cu; pd.Sp = Sp; pd.cp = cp;
+    pd.src = s->src; pd.par = s->par;
+    AsmDev &ad = v.ad;
+    ad.B = B; ad.G = G; ad.nsrc = d.nsrc; ad.nval = d.nval; ad.nnzA = (int)S->A_ci.size(); ad.nnzG = (int)S->G_ci.size();
+    ad.n = S->n; ad.p = S->p; ad.m = S->m; ad.W_rp = s->W_rp; ad.W_ci = s->W_ci; ad.W_v = s->W_v; ad.src = s->src;
+    ad.Av = D->Av; ad.Gv = D->Gv; ad.c = D->c; ad.b = D->b; ad.h = D->h; ad.c0 = s->c0;
+    StepDev &sd = v.sd;   // SCvx and GuSTO: k_extract only
+    sd.B = B; sd.G = G; sd.N = d.N; sd.nx = d.nx; sd.nu = d.nu; sd.np = d.np; sd.n = S->n; sd.vx = d.vx; sd.vu = d.vu; sd.vp = d.vp;
+    sd.q_exit = d.q_exit; sd.eps_abs = d.eps_abs; sd.eps_rel = d.eps_rel;
+    sd.Sx = Sx; sd.cx = cx; sd.Su = Su; sd.cu = cu; sd.Sp = Sp; sd.cp = cp;
+    sd.xsol = D->x; sd.pobj = D->pobj; sd.c0 = s->c0; sd.cone_status = D->status;
+    sd.xd = s->xd; sd.ud = s->ud; sd.p = s->p; sd.xn = s->xn; sd.un = s->un; sd.pn = s->pn;
+    sd.J_ref = s->J_ref; sd.J_new = s->J_new; sd.dev = s->devi; sd.imp = s->imp; sd.feas_new = s->feas;
+    sd.done = s->done; sd.status = s->status; sd.iters = s->iters; sd.nactive = s->nactive;
+    return SCPB_OK;
+}
+
+// one SCP iteration: linearize -> assemble -> cone solve -> extract -> discretize! the candidate -> step.  The whole
+// batch on the handle's stream (cs = nullptr, nb = nbp = 0; timed, and hit / nact receive the interior-point iterations
+// and the live seeds), or the chunk [b0, b0 + nbp) of whole seed groups with nb seeds of a streamed chain on cs.
+static int ptr_iteration(Solve &v, int it, cudaStream_t cs, int b0, int nb, int nbp, bool timed, int *hit, int *nact)
+{
+    scpb_ptr_s *s = v.s;
+    scpb_handle_s *h = v.h;
+    const scpb_ptr_desc &d = s->d;
+    cudaStream_t ls = cs ? cs : v.st;   // stream of the launches and copies
+    const int nbl = nb > 0 ? nb : v.B, nbn = (int)(((long long)nbl * d.N + 127) / 128);
+    auto mark = [&](int ph) { if (timed) v.mark(ph, ls); };
+    v.pd.b0 = b0; v.pd.nb = nb;
+    launch_linearize(s, v.pd, nbn, ls);
+    v.ad.b0 = b0; v.ad.nbp = nbp;
+    k_assemble<<<(unsigned)(((long long)d.nval * (nbp > 0 ? nbp : s->capB) + 255) / 256), 256, 0, ls>>>(v.ad);
+    h->launches += 2;
+    mark(1);
+    if (int r = scpb_internal_cone_run(s->cone, v.opts_at(it), s->done, cs, b0 / v.G, nbp / v.G)) return r;
+    mark(2);
+    if (hit) SCPB_CUDA(h, cudaMemcpyAsync(hit, v.D->iters, sizeof(int) * v.B, cudaMemcpyDeviceToHost, ls));
+    v.sd.iter = it; v.sd.b0 = b0; v.sd.nb = nb;
+    k_extract<<<nbn, 128, 0, ls>>>(v.sd);
+    h->launches++;
+    mark(3);
+    if (int r = run_discretize(s, v.B, v.G, s->xn, s->un, s->pn, v.cand_src, s->done, cs, b0, nb)) return r;
+    if (v.candidate)
+        if (int r = v.candidate()) return r;
+    mark(0);
+    if (nact) SCPB_CUDA(h, cudaMemsetAsync(s->nactive, 0, sizeof(int), ls));
+    if (int r = v.step(it, ls, nbl)) return r;
+    if (nact) SCPB_CUDA(h, cudaMemcpyAsync(nact, s->nactive, sizeof(int), cudaMemcpyDeviceToHost, ls));
+    mark(3);
+    return SCPB_OK;
+}
+
+// the lock-step loop: every iteration runs on the whole batch and ends when no seed is live
+static int lockstep_loop(Solve &v, int it_bound)
+{
+    scpb_handle_s *h = v.h;
+    const int B = v.B;
+    int nact = B;
+    std::vector<int> hit(B), hdone(B, 0);   // hdone: seeds that were already finished when the solver was launched (skipped)
+    for (int it = 1; it <= it_bound; it++) {
+        if (int r = ptr_iteration(v, it, nullptr, 0, 0, 0, true, hit.data(), &nact)) return r;
+        SCPB_CUDA(h, cudaStreamSynchronize(v.st));
+        for (int b = 0; b < B; b++) if (!hdone[b]) v.ipm_iters += hit[b];   // skipped seeds keep a stale count in D->iters
+        ipm_launch_stats(hit, hdone, v.total_it + 1);
+        SCPB_CUDA(h, cudaMemcpyAsync(hdone.data(), v.s->done, sizeof(int) * B, cudaMemcpyDeviceToHost, v.st));
+        SCPB_CUDA(h, cudaStreamSynchronize(v.st));
+        v.total_it++;
+        if (nact == 0) break;
     }
     return SCPB_OK;
+}
+
+// SCvx and GuSTO: the DLTV blocks of the accepted candidates become the reference linearisation
+static void take_dltv(const Solve &v)
+{
+    const scpb_ptr_desc &d = v.s->d;
+    const long long span = (long long)(d.oC - d.oA) * v.B;
+    k_scvx_take_dltv<<<(unsigned)((span + 255) / 256), 256, 0, v.st>>>(v.B, v.G, d.nsrc, d.oA, d.oC, v.s->accept, v.s->src,
+                                                                       v.s->src2);
+}
+
+// what every solve returns: the trajectories, status, iterations, cost (from Jd), deviation and feasibility, the
+// per-seed extras {host, device}, and ntiming (8, or 10 with the initial discretize!) entries of timing
+static int solve_end(Solve &v, double *xd, double *ud, double *p, int32_t *status, int32_t *iters, double *J,
+                     const double *Jd, double *deviation, int32_t *feas,
+                     std::initializer_list<std::pair<double *, const double *>> extras, double *timing, int ntiming,
+                     const char *who)
+{
+    scpb_ptr_s *s = v.s;
+    scpb_handle_s *h = v.h;
+    const scpb_ptr_desc &d = s->d;
+    cudaStream_t st = v.st;
+    const int B = v.B;
+    SCPB_CUDA(h, cudaGetLastError());
+    if (xd) SCPB_CUDA(h, cudaMemcpyAsync(xd, s->xd, sizeof(double) * B * d.N * d.nx, cudaMemcpyDeviceToHost, st));
+    if (ud) SCPB_CUDA(h, cudaMemcpyAsync(ud, s->ud, sizeof(double) * B * d.N * d.nu, cudaMemcpyDeviceToHost, st));
+    if (p) SCPB_CUDA(h, cudaMemcpyAsync(p, s->p, sizeof(double) * B * d.np, cudaMemcpyDeviceToHost, st));
+    if (status) SCPB_CUDA(h, cudaMemcpyAsync(status, s->status, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    if (iters) SCPB_CUDA(h, cudaMemcpyAsync(iters, s->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    if (J) SCPB_CUDA(h, cudaMemcpyAsync(J, Jd, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+    if (deviation) SCPB_CUDA(h, cudaMemcpyAsync(deviation, s->devi, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+    if (feas) SCPB_CUDA(h, cudaMemcpyAsync(feas, s->feas, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
+    for (const auto &e : extras)
+        if (e.first) SCPB_CUDA(h, cudaMemcpyAsync(e.first, e.second, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
+    SCPB_CUDA(h, cudaStreamSynchronize(st));
+    const std::vector<cudaEvent_t> &ev = v.evl.ev;
+    double acc[4] = {0, 0, 0, 0};
+    for (size_t i = 1; i < ev.size(); i++) {
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, ev[i - 1], ev[i]);
+        if (v.phase[i] >= 0) acc[v.phase[i]] += ms * 1e-3;
+    }
+    float tot_ms = 0.f;
+    cudaEventElapsedTime(&tot_ms, ev.front(), ev.back());
+    if (timing) {
+        timing[0] = acc[0]; timing[1] = acc[1]; timing[2] = acc[2]; timing[3] = acc[3];
+        timing[4] = tot_ms * 1e-3; timing[5] = (double)v.total_it; timing[6] = (double)v.ipm_iters;
+        timing[7] = (double)v.n_chunks;
+        if (ntiming > 8) {
+            float k1_ms = 0.f;   // the initial full-batch discretize! (K1 timed alone, before the chains fork)
+            cudaEventElapsedTime(&k1_ms, ev[0], ev[1]);
+            timing[8] = k1_ms * 1e-3; timing[9] = 0.0;
+        }
+    }
+    return ptr_check_disc_status(h, who);
 }
 
 extern "C" {
@@ -882,14 +1041,10 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
         return set_err(h, SCPB_ERR_ARG, "ptr_setup: nval does not match the cone program (%d)", desc->nval);
     if (desc->ns > 0) {
         int pns = 0, png = 0;
-        switch (h->model_id) {
-        case SCPB_MODEL_STARSHIP: pns = Constr<SCPB_MODEL_STARSHIP>::NS; png = Constr<SCPB_MODEL_STARSHIP>::NG; break;
-        case SCPB_MODEL_QUADROTOR: pns = Constr<SCPB_MODEL_QUADROTOR>::NS; png = Constr<SCPB_MODEL_QUADROTOR>::NG; break;
-        case SCPB_MODEL_FREEFLYER: pns = Constr<SCPB_MODEL_FREEFLYER>::NS; png = Constr<SCPB_MODEL_FREEFLYER>::NG; break;
-        case SCPB_MODEL_RENDEZVOUS2D:
-            pns = Constr<SCPB_MODEL_RENDEZVOUS2D>::NS; png = Constr<SCPB_MODEL_RENDEZVOUS2D>::NG; break;
-        default: break;
-        }
+        with_constr(h->model_id, true, [&](auto cp) {
+            using CP = decltype(cp);
+            if constexpr (CP::NS > 0) { pns = CP::NS; png = CP::NG; }
+        });
         if (pns != desc->ns || png != desc->ng)
             return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_setup: no constraint pack for model %d with ns=%d, ng=%d", h->model_id,
                            desc->ns, desc->ng);
@@ -928,14 +1083,13 @@ int32_t scpb_debug_constraints(scpb_handle h, int32_t B, int32_t N, int32_t ns, 
     if (B <= 0 || N <= 0 || !t_grid || !xd || !ud || !p || !s || !C || !D || !G)
         return set_err(h, SCPB_ERR_ARG, "debug_constraints: bad arguments");
     SCPB_CUDA(h, cudaSetDevice(h->device));
-    switch (h->model_id) {
-    case SCPB_MODEL_STARSHIP: return debug_constr_t<Constr<SCPB_MODEL_STARSHIP>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
-    case SCPB_MODEL_QUADROTOR: return debug_constr_t<Constr<SCPB_MODEL_QUADROTOR>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
-    case SCPB_MODEL_FREEFLYER: return debug_constr_t<Constr<SCPB_MODEL_FREEFLYER>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
-    case SCPB_MODEL_RENDEZVOUS2D:
-        return debug_constr_t<Constr<SCPB_MODEL_RENDEZVOUS2D>>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
-    default: return set_err(h, SCPB_ERR_UNSUPPORTED, "debug_constraints: model %d has no constraint pack", h->model_id);
-    }
+    int rc = SCPB_OK;
+    with_constr(h->model_id, true, [&](auto cp) {
+        using CP = decltype(cp);
+        if constexpr (CP::NS > 0) rc = debug_constr_t<CP>(h, B, N, ns, ng, t_grid, xd, ud, p, s, C, D, G);
+        else rc = set_err(h, SCPB_ERR_UNSUPPORTED, "debug_constraints: model %d has no constraint pack", h->model_id);
+    });
+    return rc;
 }
 
 int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar)
@@ -955,18 +1109,6 @@ int32_t scpb_ptr_set_par(scpb_ptr s, const double *par, int32_t npar)
     return SCPB_OK;
 }
 
-// parameter slot of the homotopy parameter of a model's constraint pack (HomSlot, csrc/constraints.cuh), -1: none
-static int pack_hom_slot(int model_id)
-{
-    switch (model_id) {
-    case SCPB_MODEL_STARSHIP: return HomSlot<Constr<SCPB_MODEL_STARSHIP>>::value;
-    case SCPB_MODEL_QUADROTOR: return HomSlot<Constr<SCPB_MODEL_QUADROTOR>>::value;
-    case SCPB_MODEL_FREEFLYER: return HomSlot<Constr<SCPB_MODEL_FREEFLYER>>::value;
-    case SCPB_MODEL_RENDEZVOUS2D: return HomSlot<Constr<SCPB_MODEL_RENDEZVOUS2D>>::value;
-    default: return -1;
-    }
-}
-
 int32_t scpb_ptr_set_homotopy(scpb_ptr s, int32_t par_index, int32_t n_grid, const double *grid, double worsen_tol)
 {
     if (!s) return SCPB_ERR_ARG;
@@ -974,7 +1116,8 @@ int32_t scpb_ptr_set_homotopy(scpb_ptr s, int32_t par_index, int32_t n_grid, con
     if (n_grid == 0) { s->hom_n = 0; s->hom_cap = 0; s->hom_slot = -1; s->hom_grid_h.clear(); return SCPB_OK; }
     if (n_grid < 0 || !grid) return set_err(h, SCPB_ERR_ARG, "ptr_set_homotopy: n_grid = %d with grid %p", n_grid, grid);
     if (s->scvx || s->gusto) return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_set_homotopy: schedules are implemented for PTR only");
-    const int slot = s->d.ns > 0 ? pack_hom_slot(s->model_id) : -1;
+    int slot = -1;   // parameter slot of the pack's homotopy parameter (HomSlot, csrc/constraints.cuh), -1: none
+    with_constr(s->model_id, s->d.ns > 0, [&](auto cp) { slot = HomSlot<decltype(cp)>::value; });
     if (slot < 0 || (par_index >= 0 && slot != par_index))
         return set_err(h, SCPB_ERR_UNSUPPORTED, "ptr_set_homotopy: the constraint pack of model %d does not read a homotopy "
                        "parameter at par[%d]", s->model_id, par_index);
@@ -1058,68 +1201,23 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
                        int32_t *iters, double *J, double *deviation, int32_t *feas, double *timing)
 {
     if (!s) return SCPB_ERR_ARG;
-    scpb_handle_s *h = s->h;
-    if (B <= 0 || !xd0 || !ud0 || !p0) return set_err(h, SCPB_ERR_ARG, "ptr_solve: bad arguments");
-    SCPB_CUDA(h, cudaSetDevice(h->device));
-    ptr_select_model(s);
-    SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
-    const scpb_ptr_desc &d = s->d;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
-    int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
+    Solve v;
+    int rc = solve_begin(v, s, B, xd0, ud0, p0, opts, "ptr_solve");
     if (rc) return rc;
-    if ((rc = ptr_reserve(s, B, G))) return rc;
+    scpb_handle_s *h = s->h;
+    const scpb_ptr_desc &d = s->d;
+    cudaStream_t st = v.st;
+    const int G = v.G, Bpad = s->capB;
+    IpmData *D = v.D;
+    StepDev &sd = v.sd;
+    if (D->warm) SCPB_CUDA(h, cudaMemsetAsync(D->warm, 0, sizeof(int) * s->capB, st));   // warm points of an earlier batch are not this batch's
     const bool hom = s->hom_n > 0;
-    if (hom) {
-        if ((int)s->hom_beta_h.size() != B)
-            return set_err(h, SCPB_ERR_STATE, "ptr_solve: the homotopy schedule has %d update thresholds for %d seeds "
-                           "(scpb_ptr_set_homotopy_beta)", (int)s->hom_beta_h.size(), B);
-        if ((rc = hom_reserve(s, s->capB))) return rc;
-    }
     // a seed with a schedule can run iter_max + (n_grid - 1)(iter_max - 1) iterations (every update extends its
     // iter_max by the iterations since the previous one)
     const int it_bound = hom ? s->hom_cap : d.iter_max;
-    IpmData *D = scpb_internal_cone_data(s->cone);
-    const ConeSymbolic *S = scpb_internal_cone_sym(s->cone);
-    IpmOpts o_ = scpb_internal_make_opts(opts);
-    scpb_internal_relax_refinement(o_);
-    const IpmOpts o = o_;
-    cudaStream_t st = h->stream;
-    const size_t nX = (size_t)B * d.N * d.nx, nU = (size_t)B * d.N * d.nu, nP = (size_t)B * d.np;
-    SCPB_CUDA(h, cudaMemcpyAsync(s->xd, xd0, sizeof(double) * nX, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->ud, ud0, sizeof(double) * nU, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->p, p0, sizeof(double) * nP, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->src, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->done, 0, sizeof(int) * s->capB, st));
-    if (D->warm) SCPB_CUDA(h, cudaMemsetAsync(D->warm, 0, sizeof(int) * s->capB, st));   // warm points of an earlier batch are not this batch's
-    SCPB_CUDA(h, cudaMemsetAsync(s->iters, 0, sizeof(int) * s->capB, st));
-    std::vector<int> init_status(s->capB, 1);
-    SCPB_CUDA(h, cudaMemcpyAsync(s->status, init_status.data(), sizeof(int) * s->capB, cudaMemcpyHostToDevice, st));
-    std::vector<double> nanv(s->capB, nan(""));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->J_ref, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->devi, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-
-    const size_t nsc = (size_t)(d.nx + d.nu + d.np);
-    const double *Sx = s->scale, *Su = Sx + d.nx, *Sp = Su + d.nu, *cx = s->scale + nsc, *cu = cx + d.nx, *cp = cu + d.nu;
-    PtrDev pd{};
-    pd.B = B; pd.G = G; pd.N = d.N; pd.nx = d.nx; pd.nu = d.nu; pd.np = d.np; pd.ns = d.ns;
-    pd.nsrc = d.nsrc; pd.oC = d.oC; pd.oD = d.oD; pd.oG = d.oG; pd.ors = d.ors; pd.oxh = d.oxh; pd.ouh = d.ouh; pd.oph = d.oph;
-    pd.t_grid = s->tgrid; pd.Sx = Sx; pd.cx = cx; pd.Su = Su; pd.cu = cu; pd.Sp = Sp; pd.cp = cp;
-    pd.src = s->src; pd.par = s->par;
-    AsmDev ad{};
-    ad.B = B; ad.G = G; ad.nsrc = d.nsrc; ad.nval = d.nval; ad.nnzA = (int)S->A_ci.size(); ad.nnzG = (int)S->G_ci.size();
-    ad.n = S->n; ad.p = S->p; ad.m = S->m; ad.W_rp = s->W_rp; ad.W_ci = s->W_ci; ad.W_v = s->W_v; ad.src = s->src;
-    ad.Av = D->Av; ad.Gv = D->Gv; ad.c = D->c; ad.b = D->b; ad.h = D->h; ad.c0 = s->c0;
-    StepDev sd{};
-    sd.B = B; sd.G = G; sd.N = d.N; sd.nx = d.nx; sd.nu = d.nu; sd.np = d.np; sd.n = S->n; sd.vx = d.vx; sd.vu = d.vu; sd.vp = d.vp;
-    sd.q_exit = d.q_exit; sd.eps_abs = d.eps_abs; sd.eps_rel = d.eps_rel;
-    sd.Sx = Sx; sd.cx = cx; sd.Su = Su; sd.cu = cu; sd.Sp = Sp; sd.cp = cp;
-    sd.xsol = D->x; sd.pobj = D->pobj; sd.c0 = s->c0; sd.cone_status = D->status;
-    sd.xd = s->xd; sd.ud = s->ud; sd.p = s->p; sd.xn = s->xn; sd.un = s->un; sd.pn = s->pn;
-    sd.J_ref = s->J_ref; sd.J_new = s->J_new; sd.dev = s->devi; sd.imp = s->imp; sd.feas_new = s->feas;
-    sd.done = s->done; sd.status = s->status; sd.iters = s->iters; sd.nactive = s->nactive;
     s->last_B = B; s->last_cap = hom ? s->hom_cap : 0;
     if (hom) {
-        pd.kappa = s->hom_kappa;
+        v.pd.kappa = s->hom_kappa;
         sd.hom_n = s->hom_n; sd.hist_cap = s->hom_cap; sd.worsen_tol = s->hom_wtol;
         sd.hom_grid = s->hom_grid; sd.hom_beta = s->hom_beta;
         sd.hom_idx = s->hom_idx; sd.hom_last = s->hom_last; sd.hom_itmax = s->hom_itmax; sd.hom_kappa = s->hom_kappa;
@@ -1129,40 +1227,39 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
         k_hom_init<<<(unsigned)((n_init + 127) / 128), 128, 0, st>>>(sd, d.iter_max, B);
         h->launches++;
     }
+    // interior-point warm start across PTR iterations: from iteration warm_from on, every seed starts the interior-point
+    // method from the warm point its previous solve stored (the subproblems of consecutive PTR iterations differ little).
+    // Built and correct, but not faster on the bench workload (the median iteration count of the later subproblems drops
+    // from 37 to 28-33, the slowest seed of a launch needs more) -- opt-in with SCPB_WARM=1 (SCPB_NO_WARM=1 turns it off)
+    const bool no_warm = getenv("SCPB_WARM") == nullptr || getenv("SCPB_NO_WARM") != nullptr;
+    int warm_from = 5;   // SCPB_WARM_FROM
+    if (const char *e = getenv("SCPB_WARM_FROM")) warm_from = atoi(e);
+    IpmOpts o = v.o;
+    scpb_internal_relax_refinement(o);
+    v.opts_at = [=](int it) { IpmOpts ow = o; ow.warm = (it >= warm_from && !no_warm) ? 1 : 0; return ow; };
+    v.step = [&](int, cudaStream_t ls, int nb) -> int {
+        k_ptr_step<<<(nb + 127) / 128, 128, 0, ls>>>(sd);
+        h->launches++;
+        return SCPB_OK;
+    };
 
-    // phase timers (the reference's keys: discretize / formulate / solve / overhead, scp.jl:177-178,990-995)
-    EventList evl;
-    std::vector<cudaEvent_t> &ev = evl.ev;
-    auto mark = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); ev.push_back(e); };
-    std::vector<int> phase;   // phase id of the interval that ENDS at event i
-    mark(); phase.push_back(-1);
+    v.mark(-1, st);
     if ((rc = run_discretize(s, B, G, s->xd, s->ud, s->p))) return rc;   // generate_initial_guess -> discretize!
-    mark(); phase.push_back(0);
-    const int nbn = (int)(((long long)B * d.N + 127) / 128);
-    const int Bpad = s->capB;
-    int it = 1, nact = B, total_it = 0;
-    long long ipm_iters = 0;
-    // ---- streamed chains (default): seeds are independent, so the batch is cut into chunks of whole seed groups and every
+    v.mark(0, st);
+    // ---- streamed chains: seeds are independent, so the batch is cut into chunks of whole seed groups and every
     // chunk runs ITS OWN sequence of iter_max PTR iterations on its own stream, with no host synchronisation in between: a
     // finished seed turns its share of every later kernel into a no-op (skip masks), a finished chunk costs a few empty
     // launches.  In lock-step every solver launch lasts as long as the slowest of ALL seeds (measured on the bench:
     // median 37, max 73 interior-point iterations in the later subproblems); streamed, a chunk only waits for its own seeds
     // and the batch takes max-over-chunks of the sums instead of the sum of the maxima.  SCPB_PTR_CHUNKS=<n> sets the
-    // number of chunks (default 64 <= concurrent-kernel limit; 0 or 1 = lock-step loop below, which also serves the
-    // SCPB_IPM_STATS diagnostic).
-    // interior-point warm start across PTR iterations: built and correct, but not faster on the bench workload (the median
-    // iteration count of the later subproblems drops from 37 to 28-33, the slowest seed of a launch needs more) -- opt-in
-    // with SCPB_WARM=1
-    const bool no_warm = getenv("SCPB_WARM") == nullptr || getenv("SCPB_NO_WARM") != nullptr;
-    int warm_from = 5;   // first PTR iteration whose subproblems start from the stored warm points (SCPB_WARM_FROM)
-    if (const char *e = getenv("SCPB_WARM_FROM")) warm_from = atoi(e);
+    // number of chunks; 0 or 1 (the default, SCPB_PTR_DEFAULT_CHUNKS = 0) runs the lock-step loop, which also serves the
+    // SCPB_IPM_STATS diagnostic.
     int max_chunks = SCPB_PTR_DEFAULT_CHUNKS;
     if (const char *e = getenv("SCPB_PTR_CHUNKS")) max_chunks = atoi(e);
     const int ng_all = (B + G - 1) / G;
-    int n_chunks = 0;
     if (max_chunks > 1 && ng_all >= 2 && !getenv("SCPB_IPM_STATS")) {
         const int cg = (ng_all + max_chunks - 1) / max_chunks;   // seed groups per chunk
-        n_chunks = (ng_all + cg - 1) / cg;
+        const int n_chunks = v.n_chunks = (ng_all + cg - 1) / cg;
         while ((int)s->chunk_streams.size() < n_chunks) {
             cudaStream_t q = nullptr;
             SCPB_CUDA(h, cudaStreamCreateWithFlags(&q, cudaStreamNonBlocking));
@@ -1176,41 +1273,17 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
         cudaEvent_t e_fork = sync_event();
         SCPB_CUDA(h, cudaEventRecord(e_fork, st));
         for (int c = 0; c < n_chunks; c++) SCPB_CUDA(h, cudaStreamWaitEvent(s->chunk_streams[c], e_fork, 0));
-        auto mark0 = [&](int ph) { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, s->chunk_streams[0]); ev.push_back(e); phase.push_back(ph); };
-        mark0(-1);   // chunk 0 carries the phase timers: its own chain is one of the n_chunks concurrent critical paths
+        v.mark(-1, s->chunk_streams[0]);   // chunk 0 carries the phase timers: its own chain is one of the n_chunks concurrent critical paths
         // iteration `it` of chunk c's chain
-        auto enqueue = [&](int c, int it) -> int {
-            cudaStream_t cs = s->chunk_streams[c];
+        auto enqueue = [&](int c, int it) {
             const int b0 = c * cg * G;
             const int nbp = std::min(cg * G, Bpad - b0), nb = std::min(nbp, B - b0);
-            const int nbn_c = (int)(((long long)nb * d.N + 127) / 128);
-            pd.b0 = b0; pd.nb = nb;
-            launch_linearize(s, pd, nbn_c, cs);
-            ad.b0 = b0; ad.nbp = nbp;
-            k_assemble<<<(unsigned)(((long long)d.nval * nbp + 255) / 256), 256, 0, cs>>>(ad);
-            h->launches += 2;
-            if (c == 0) mark0(1);
-            {
-                IpmOpts ow = o;
-                ow.warm = (it >= warm_from && !no_warm) ? 1 : 0;
-                if (int r = scpb_internal_cone_run(s->cone, ow, s->done, cs, b0 / G, nbp / G)) return r;
-            }
-            if (c == 0) mark0(2);
-            sd.iter = it; sd.b0 = b0; sd.nb = nb;
             sd.ndone = hom ? s->d_chunk_done + c : nullptr;
-            k_extract<<<nbn_c, 128, 0, cs>>>(sd);
-            h->launches++;
-            if (c == 0) mark0(3);
-            if (int r = run_discretize(s, B, G, s->xn, s->un, s->pn, nullptr, s->done, cs, b0, nb)) return r;
-            if (c == 0) mark0(0);
-            k_ptr_step<<<(nb + 127) / 128, 128, 0, cs>>>(sd);
-            h->launches++;
-            if (c == 0) mark0(3);
-            return SCPB_OK;
+            return ptr_iteration(v, it, s->chunk_streams[c], b0, nb, nbp, c == 0, nullptr, nullptr);
         };
         auto chunk_seeds = [&](int c) { const int b0 = c * cg * G; return std::min(std::min(cg * G, Bpad - b0), B - b0); };
         if (!hom) {
-            for (it = 1; it <= it_bound; it++)
+            for (int it = 1; it <= it_bound; it++)
                 for (int c = 0; c < n_chunks; c++)
                     if (chunk_seeds(c) > 0 && (rc = enqueue(c, it))) return rc;
         } else {
@@ -1265,76 +1338,18 @@ int32_t scpb_ptr_solve(scpb_ptr s, int32_t B, const double *xd0, const double *u
             SCPB_CUDA(h, cudaEventRecord(e, s->chunk_streams[c]));
             SCPB_CUDA(h, cudaStreamWaitEvent(st, e, 0));
         }
-        mark(); phase.push_back(-1);
+        v.mark(-1, st);
         unsigned long long tot_ipm = 0;
         SCPB_CUDA(h, cudaMemcpyAsync(&tot_ipm, s->d_ipm_total, sizeof tot_ipm, cudaMemcpyDeviceToHost, st));
         std::vector<int> hiters(B);
         SCPB_CUDA(h, cudaMemcpyAsync(hiters.data(), s->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
         SCPB_CUDA(h, cudaStreamSynchronize(st));
-        ipm_iters = (long long)tot_ipm;
-        for (int b = 0; b < B; b++) total_it = std::max(total_it, hiters[b]);   // the longest chain
-        it = it_bound + 1;   // skip the lock-step loop
+        v.ipm_iters = (long long)tot_ipm;
+        for (int b = 0; b < B; b++) v.total_it = std::max(v.total_it, hiters[b]);   // the longest chain
+    } else if ((rc = lockstep_loop(v, it_bound))) {
+        return rc;
     }
-    std::vector<int> hit(B), hdone(B, 0);   // hdone: seeds that were already finished when the solver was launched (skipped)
-    for (; it <= it_bound; it++) {
-        launch_linearize(s, pd, nbn, st);
-        const long long tot = (long long)d.nval * Bpad;
-        k_assemble<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ad);
-        h->launches += 2;
-        mark(); phase.push_back(1);
-        {   // from the second subproblem on every seed starts the interior-point method from the warm point its previous
-            // solve stored (the subproblems of consecutive PTR iterations differ little); SCPB_NO_WARM=1 turns it off
-            IpmOpts ow = o;
-            ow.warm = (it >= warm_from && !no_warm) ? 1 : 0;
-            if ((rc = scpb_internal_cone_run(s->cone, ow, s->done, nullptr, 0, 0))) return rc;
-        }
-        mark(); phase.push_back(2);
-        SCPB_CUDA(h, cudaMemcpyAsync(hit.data(), D->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        sd.iter = it;
-        k_extract<<<nbn, 128, 0, st>>>(sd);
-        h->launches++;
-        mark(); phase.push_back(3);
-        if ((rc = run_discretize(s, B, G, s->xn, s->un, s->pn, nullptr, s->done))) return rc;
-        mark(); phase.push_back(0);
-        SCPB_CUDA(h, cudaMemsetAsync(s->nactive, 0, sizeof(int), st));
-        k_ptr_step<<<(B + 127) / 128, 128, 0, st>>>(sd);
-        h->launches++;
-        SCPB_CUDA(h, cudaMemcpyAsync(&nact, s->nactive, sizeof(int), cudaMemcpyDeviceToHost, st));
-        mark(); phase.push_back(3);
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        for (int b = 0; b < B; b++) if (!hdone[b]) ipm_iters += hit[b];   // skipped seeds keep a stale count in D->iters
-        ipm_launch_stats(hit, hdone, total_it + 1);
-        SCPB_CUDA(h, cudaMemcpyAsync(hdone.data(), s->done, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        total_it++;
-        if (nact == 0) break;
-    }
-    SCPB_CUDA(h, cudaGetLastError());
-    if (xd) SCPB_CUDA(h, cudaMemcpyAsync(xd, s->xd, sizeof(double) * nX, cudaMemcpyDeviceToHost, st));
-    if (ud) SCPB_CUDA(h, cudaMemcpyAsync(ud, s->ud, sizeof(double) * nU, cudaMemcpyDeviceToHost, st));
-    if (p) SCPB_CUDA(h, cudaMemcpyAsync(p, s->p, sizeof(double) * nP, cudaMemcpyDeviceToHost, st));
-    if (status) SCPB_CUDA(h, cudaMemcpyAsync(status, s->status, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (iters) SCPB_CUDA(h, cudaMemcpyAsync(iters, s->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (J) SCPB_CUDA(h, cudaMemcpyAsync(J, s->J_ref, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (deviation) SCPB_CUDA(h, cudaMemcpyAsync(deviation, s->devi, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (feas) SCPB_CUDA(h, cudaMemcpyAsync(feas, s->feas, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    SCPB_CUDA(h, cudaStreamSynchronize(st));
-    double acc[4] = {0, 0, 0, 0};
-    for (size_t i = 1; i < ev.size(); i++) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, ev[i - 1], ev[i]);
-        if (phase[i] >= 0) acc[phase[i]] += ms * 1e-3;
-    }
-    float tot_ms = 0.f;
-    cudaEventElapsedTime(&tot_ms, ev.front(), ev.back());
-    if (timing) {
-        timing[0] = acc[0]; timing[1] = acc[1]; timing[2] = acc[2]; timing[3] = acc[3];
-        timing[4] = tot_ms * 1e-3; timing[5] = (double)total_it; timing[6] = (double)ipm_iters; timing[7] = (double)n_chunks;
-        float k1_ms = 0.f;   // the initial full-batch discretize! (K1 timed alone, before the chains fork)
-        cudaEventElapsedTime(&k1_ms, ev[0], ev[1]);
-        timing[8] = k1_ms * 1e-3; timing[9] = 0.0;
-    }
-    return ptr_check_disc_status(h, "ptr_solve");
+    return solve_end(v, xd, ud, p, status, iters, J, s->J_ref, deviation, feas, {}, timing, 10, "ptr_solve");
 }
 
 int32_t scpb_scvx_attach(scpb_ptr s, const scpb_scvx_desc *desc, const int32_t *Q_rowptr, const int32_t *Q_colind,
@@ -1346,6 +1361,11 @@ int32_t scpb_scvx_attach(scpb_ptr s, const scpb_scvx_desc *desc, const int32_t *
     const scpb_ptr_desc &d = s->d;
     if (s->hom_n > 0) return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: the problem has an in-loop homotopy schedule (PTR only)");
     if (d.method != SCPB_FOH) return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: SCvx runs with FOH discretization only");
+    bool pack_ok = false;
+    with_constr(s->model_id, d.ns > 0, [&](auto cp) { pack_ok = scvx_has_pack<decltype(cp)>; });
+    if (!pack_ok)
+        return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_attach: SCvx has no penalty for the constraint pack of model %d",
+                       s->model_id);
     if (desc->oeta <= 0 || desc->oeta >= d.nsrc || desc->n_ic < 0 || desc->n_tc < 0)
         return set_err(h, SCPB_ERR_ARG, "scvx_attach: bad descriptor (oeta=%d)", desc->oeta);
     const int nq = 1 + desc->n_ic + desc->n_tc, nnz = Q_rowptr[nq];
@@ -1372,149 +1392,64 @@ int32_t scpb_scvx_solve(scpb_ptr s, int32_t B, const double *xd0, const double *
                         int32_t *iters, double *J, double *deviation, int32_t *feas, double *eta, double *timing)
 {
     if (!s) return SCPB_ERR_ARG;
-    scpb_handle_s *h = s->h;
-    if (!s->scvx) return set_err(h, SCPB_ERR_STATE, "scvx_solve: call scpb_scvx_attach first");
-    if (B <= 0 || !xd0 || !ud0 || !p0) return set_err(h, SCPB_ERR_ARG, "scvx_solve: bad arguments");
-    SCPB_CUDA(h, cudaSetDevice(h->device));
-    ptr_select_model(s);
-    SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
-    const scpb_ptr_desc &d = s->d;
-    const scpb_scvx_desc &v = s->sv;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
-    int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
+    if (!s->scvx) return set_err(s->h, SCPB_ERR_STATE, "scvx_solve: call scpb_scvx_attach first");
+    Solve v;
+    int rc = solve_begin(v, s, B, xd0, ud0, p0, opts, "scvx_solve");
     if (rc) return rc;
-    if ((rc = ptr_reserve(s, B, G))) return rc;
-    IpmData *D = scpb_internal_cone_data(s->cone);
-    const ConeSymbolic *S = scpb_internal_cone_sym(s->cone);
-    const IpmOpts o = scpb_internal_make_opts(opts);
-    cudaStream_t st = h->stream;
-    const size_t nX = (size_t)B * d.N * d.nx, nU = (size_t)B * d.N * d.nu, nP = (size_t)B * d.np;
-    SCPB_CUDA(h, cudaMemcpyAsync(s->xd, xd0, sizeof(double) * nX, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->ud, ud0, sizeof(double) * nU, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->p, p0, sizeof(double) * nP, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->src, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->src2, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->done, 0, sizeof(int) * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->iters, 0, sizeof(int) * s->capB, st));
-    std::vector<int> init_status(s->capB, 1);
-    SCPB_CUDA(h, cudaMemcpyAsync(s->status, init_status.data(), sizeof(int) * s->capB, cudaMemcpyHostToDevice, st));
-    std::vector<double> nanv(s->capB, nan(""));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->devi, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->J_out, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->eta, v.eta_init, s->capB);
+    scpb_handle_s *h = s->h;
+    const scpb_ptr_desc &d = s->d;
+    const scpb_scvx_desc &sv = s->sv;
+    cudaStream_t st = v.st;
+    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->eta, sv.eta_init, s->capB);
     h->launches++;
-
-    const size_t nsc = (size_t)(d.nx + d.nu + d.np);
-    const double *Sx = s->scale, *Su = Sx + d.nx, *Sp = Su + d.nu, *cx = s->scale + nsc, *cu = cx + d.nx, *cp = cu + d.nu;
-    PtrDev pd{};
-    pd.B = B; pd.G = G; pd.N = d.N; pd.nx = d.nx; pd.nu = d.nu; pd.np = d.np; pd.ns = d.ns;
-    pd.nsrc = d.nsrc; pd.oC = d.oC; pd.oD = d.oD; pd.oG = d.oG; pd.ors = d.ors; pd.oxh = d.oxh; pd.ouh = d.ouh; pd.oph = d.oph;
-    pd.t_grid = s->tgrid; pd.Sx = Sx; pd.cx = cx; pd.Su = Su; pd.cu = cu; pd.Sp = Sp; pd.cp = cp;
-    pd.src = s->src; pd.par = s->par; pd.eta = s->eta; pd.oeta = v.oeta;
-    AsmDev ad{};
-    ad.B = B; ad.G = G; ad.nsrc = d.nsrc; ad.nval = d.nval; ad.nnzA = (int)S->A_ci.size(); ad.nnzG = (int)S->G_ci.size();
-    ad.n = S->n; ad.p = S->p; ad.m = S->m; ad.W_rp = s->W_rp; ad.W_ci = s->W_ci; ad.W_v = s->W_v; ad.src = s->src;
-    ad.Av = D->Av; ad.Gv = D->Gv; ad.c = D->c; ad.b = D->b; ad.h = D->h; ad.c0 = s->c0;
-    StepDev sd{};   // k_extract only
-    sd.B = B; sd.G = G; sd.N = d.N; sd.nx = d.nx; sd.nu = d.nu; sd.np = d.np; sd.n = S->n; sd.vx = d.vx; sd.vu = d.vu; sd.vp = d.vp;
-    sd.q_exit = d.q_exit; sd.eps_abs = d.eps_abs; sd.eps_rel = d.eps_rel;
-    sd.Sx = Sx; sd.cx = cx; sd.Su = Su; sd.cu = cu; sd.Sp = Sp; sd.cp = cp;
-    sd.xsol = D->x; sd.pobj = D->pobj; sd.c0 = s->c0; sd.cone_status = D->status;
-    sd.xd = s->xd; sd.ud = s->ud; sd.p = s->p; sd.xn = s->xn; sd.un = s->un; sd.pn = s->pn;
-    sd.J_ref = s->J_ref; sd.J_new = s->J_new; sd.dev = s->devi; sd.imp = s->imp; sd.feas_new = s->feas;
-    sd.done = s->done; sd.status = s->status; sd.iters = s->iters; sd.nactive = s->nactive;
+    v.pd.eta = s->eta; v.pd.oeta = sv.oeta;
+    const StepDev &sd = v.sd;
     ScvxDev cv{};
-    cv.B = B; cv.G = G; cv.N = d.N; cv.nx = d.nx; cv.nu = d.nu; cv.np = d.np; cv.n_ic = v.n_ic; cv.n_tc = v.n_tc;
-    cv.vx = d.vx; cv.vu = d.vu; cv.vp = d.vp; cv.q_exit = d.q_exit; cv.iter_max = d.iter_max; cv.nsrc = d.nsrc;
-    cv.dltv_lo = d.oA; cv.dltv_hi = d.oC;
-    cv.lam = v.lam; cv.rho_0 = v.rho_0; cv.rho_1 = v.rho_1; cv.rho_2 = v.rho_2; cv.beta_sh = v.beta_sh; cv.beta_gr = v.beta_gr;
-    cv.eta_lb = v.eta_lb; cv.eta_ub = v.eta_ub; cv.eps_abs = d.eps_abs; cv.eps_rel = d.eps_rel;
+    cv.B = B; cv.N = d.N; cv.nx = d.nx; cv.nu = d.nu; cv.np = d.np; cv.n_ic = sv.n_ic; cv.n_tc = sv.n_tc;
+    cv.vx = d.vx; cv.vu = d.vu; cv.vp = d.vp; cv.q_exit = d.q_exit; cv.iter_max = d.iter_max;
+    cv.lam = sv.lam; cv.rho_0 = sv.rho_0; cv.rho_1 = sv.rho_1; cv.rho_2 = sv.rho_2; cv.beta_sh = sv.beta_sh; cv.beta_gr = sv.beta_gr;
+    cv.eta_lb = sv.eta_lb; cv.eta_ub = sv.eta_ub; cv.eps_abs = d.eps_abs; cv.eps_rel = d.eps_rel;
     cv.Q_rp = s->Q_rp; cv.Q_ci = s->Q_ci; cv.Q_v = s->Q_v; cv.Q_c = s->Q_c;
-    cv.Sx = Sx; cv.cx = cx; cv.Su = Su; cv.cu = cu; cv.Sp = Sp; cv.cp = cp; cv.t_grid = s->tgrid; cv.defect = s->defect;
-    cv.par = s->par;
+    cv.Sx = sd.Sx; cv.cx = sd.cx; cv.Su = sd.Su; cv.cu = sd.cu; cv.Sp = sd.Sp; cv.cp = sd.cp; cv.t_grid = s->tgrid;
+    cv.defect = s->defect; cv.par = s->par;
     cv.xd = s->xd; cv.ud = s->ud; cv.p = s->p; cv.xn = s->xn; cv.un = s->un; cv.pn = s->pn;
     cv.J_ref = s->J_ref; cv.J_new = s->J_new; cv.L_new = s->L_new; cv.J_out = s->J_out; cv.eta = s->eta; cv.dev = s->devi;
-    cv.cone_status = D->status; cv.feas_new = s->feas;
+    cv.cone_status = v.D->status; cv.feas_new = s->feas;
     cv.done = s->done; cv.status = s->status; cv.iters = s->iters; cv.nactive = s->nactive; cv.accept = s->accept;
-    cv.src = s->src; cv.src2 = s->src2;
-    const bool pack = (s->model_id == SCPB_MODEL_STARSHIP && d.ns > 0);
-    auto cost = [&](const double *X, const double *U, const double *P, double *Jd, double *Ld) {
-        if (pack) k_scvx_cost<Constr<SCPB_MODEL_STARSHIP>><<<(B + 63) / 64, 64, 0, st>>>(cv, X, U, P, Jd, Ld);
-        else k_scvx_cost<Constr<0>><<<(B + 63) / 64, 64, 0, st>>>(cv, X, U, P, Jd, Ld);
-        h->launches++;
+    // a pack without a penalty is refused, not run with its rows of J left unwritten (scpb_scvx_attach refuses it first)
+    auto cost = [&](const double *X, const double *U, const double *P, double *Jd, double *Ld) -> int {
+        bool launched = false;
+        with_constr(s->model_id, d.ns > 0, [&](auto cp) {
+            using CP = decltype(cp);
+            if constexpr (scvx_has_pack<CP>) {
+                k_scvx_cost<CP><<<(B + 63) / 64, 64, 0, st>>>(cv, X, U, P, Jd, Ld);
+                h->launches++;
+                launched = true;
+            }
+        });
+        if (!launched)
+            return set_err(h, SCPB_ERR_UNSUPPORTED, "scvx_solve: SCvx has no penalty for the constraint pack of model %d",
+                           s->model_id);
+        return SCPB_OK;
     };
-
-    EventList evl;
-    std::vector<cudaEvent_t> &ev = evl.ev;
-    auto mark = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); ev.push_back(e); };
-    std::vector<int> phase;
-    mark(); phase.push_back(-1);
-    // generate_initial_guess: SubproblemSolution(x, u, p, 0, pbm) = discretize! + nonlinear cost (scvx.jl:560-568, 392-394)
-    if ((rc = run_discretize(s, B, G, s->xd, s->ud, s->p))) return rc;
-    cost(s->xd, s->ud, s->p, s->J_ref, s->L_new);
-    mark(); phase.push_back(0);
-    const int nbn = (int)(((long long)B * d.N + 127) / 128);
-    const int Bpad = s->capB;
-    int it = 1, nact = B, total_it = 0;
-    long long ipm_iters = 0;
-    std::vector<int> hit(B), hdone(B, 0);   // hdone: seeds that were already finished when the solver was launched (skipped)
-    const long long span = (long long)(d.oC - d.oA) * B;
-    for (; it <= d.iter_max; it++) {
-        if (pack) k_linearize<Constr<SCPB_MODEL_STARSHIP>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-        else k_linearize<Constr<0>><<<nbn, 128, 0, st>>>(pd, s->xd, s->ud, s->p);
-        const long long tot = (long long)d.nval * Bpad;
-        k_assemble<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ad);
-        h->launches += 2;
-        mark(); phase.push_back(1);
-        if ((rc = scpb_internal_cone_run(s->cone, o, s->done, nullptr, 0, 0))) return rc;
-        mark(); phase.push_back(2);
-        SCPB_CUDA(h, cudaMemcpyAsync(hit.data(), D->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        sd.iter = it;
-        k_extract<<<nbn, 128, 0, st>>>(sd);
-        h->launches++;
-        mark(); phase.push_back(3);
-        if ((rc = run_discretize(s, B, G, s->xn, s->un, s->pn, s->src2, s->done))) return rc;   // candidate: DLTV into src2
-        cost(s->xn, s->un, s->pn, s->J_new, s->L_new);
-        mark(); phase.push_back(0);
-        SCPB_CUDA(h, cudaMemsetAsync(s->nactive, 0, sizeof(int), st));
+    v.opts_at = [&](int) { return v.o; };
+    v.cand_src = s->src2;
+    v.candidate = [&]() { return cost(s->xn, s->un, s->pn, s->J_new, s->L_new); };
+    v.step = [&](int it, cudaStream_t, int) -> int {
         cv.iter = it;
         k_scvx_step<<<(B + 127) / 128, 128, 0, st>>>(cv);
-        k_scvx_take_dltv<<<(unsigned)((span + 255) / 256), 256, 0, st>>>(cv);
+        take_dltv(v);
         h->launches += 2;
-        SCPB_CUDA(h, cudaMemcpyAsync(&nact, s->nactive, sizeof(int), cudaMemcpyDeviceToHost, st));
-        mark(); phase.push_back(3);
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        for (int b = 0; b < B; b++) if (!hdone[b]) ipm_iters += hit[b];   // skipped seeds keep a stale count in D->iters
-        ipm_launch_stats(hit, hdone, total_it + 1);
-        SCPB_CUDA(h, cudaMemcpyAsync(hdone.data(), s->done, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        total_it++;
-        if (nact == 0) break;
-    }
-    SCPB_CUDA(h, cudaGetLastError());
-    if (xd) SCPB_CUDA(h, cudaMemcpyAsync(xd, s->xd, sizeof(double) * nX, cudaMemcpyDeviceToHost, st));
-    if (ud) SCPB_CUDA(h, cudaMemcpyAsync(ud, s->ud, sizeof(double) * nU, cudaMemcpyDeviceToHost, st));
-    if (p) SCPB_CUDA(h, cudaMemcpyAsync(p, s->p, sizeof(double) * nP, cudaMemcpyDeviceToHost, st));
-    if (status) SCPB_CUDA(h, cudaMemcpyAsync(status, s->status, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (iters) SCPB_CUDA(h, cudaMemcpyAsync(iters, s->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (J) SCPB_CUDA(h, cudaMemcpyAsync(J, s->J_out, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (deviation) SCPB_CUDA(h, cudaMemcpyAsync(deviation, s->devi, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (feas) SCPB_CUDA(h, cudaMemcpyAsync(feas, s->feas, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (eta) SCPB_CUDA(h, cudaMemcpyAsync(eta, s->eta, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    SCPB_CUDA(h, cudaStreamSynchronize(st));
-    double acc[4] = {0, 0, 0, 0};
-    for (size_t i = 1; i < ev.size(); i++) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, ev[i - 1], ev[i]);
-        if (phase[i] >= 0) acc[phase[i]] += ms * 1e-3;
-    }
-    float tot_ms = 0.f;
-    cudaEventElapsedTime(&tot_ms, ev.front(), ev.back());
-    if (timing) {
-        timing[0] = acc[0]; timing[1] = acc[1]; timing[2] = acc[2]; timing[3] = acc[3];
-        timing[4] = tot_ms * 1e-3; timing[5] = (double)total_it; timing[6] = (double)ipm_iters; timing[7] = 0.0;
-    }
-    return ptr_check_disc_status(h, "scvx_solve");
+        return SCPB_OK;
+    };
+
+    v.mark(-1, st);
+    // generate_initial_guess: SubproblemSolution(x, u, p, 0, pbm) = discretize! + nonlinear cost (scvx.jl:560-568, 392-394)
+    if ((rc = run_discretize(s, B, v.G, s->xd, s->ud, s->p))) return rc;
+    if ((rc = cost(s->xd, s->ud, s->p, s->J_ref, s->L_new))) return rc;
+    v.mark(0, st);
+    if ((rc = lockstep_loop(v, d.iter_max))) return rc;
+    return solve_end(v, xd, ud, p, status, iters, J, s->J_out, deviation, feas, {{eta, s->eta}}, timing, 8, "scvx_solve");
 }
 
 int32_t scpb_gusto_attach(scpb_ptr s, const scpb_gusto_desc *desc, const int32_t *Q_rowptr, const int32_t *Q_colind,
@@ -1560,145 +1495,51 @@ int32_t scpb_gusto_solve(scpb_ptr s, int32_t B, const double *xd0, const double 
                          double *timing)
 {
     if (!s) return SCPB_ERR_ARG;
-    scpb_handle_s *h = s->h;
-    if (!s->gusto) return set_err(h, SCPB_ERR_STATE, "gusto_solve: call scpb_gusto_attach first");
-    if (B <= 0 || !xd0 || !ud0 || !p0) return set_err(h, SCPB_ERR_ARG, "gusto_solve: bad arguments");
-    SCPB_CUDA(h, cudaSetDevice(h->device));
-    ptr_select_model(s);
-    SCPB_CUDA(h, cudaMemsetAsync(h->d_status, 0, sizeof(int), h->stream));
-    const scpb_ptr_desc &d = s->d;
-    const scpb_gusto_desc &v = s->gv;
-    const int G = scpb_internal_pick_group(B, opts ? opts->group : 0, h->sms);
-    int rc = scpb_internal_cone_reserve(s->cone, B, G, opts ? opts->lanes : 0);
+    if (!s->gusto) return set_err(s->h, SCPB_ERR_STATE, "gusto_solve: call scpb_gusto_attach first");
+    Solve v;
+    int rc = solve_begin(v, s, B, xd0, ud0, p0, opts, "gusto_solve");
     if (rc) return rc;
-    if ((rc = ptr_reserve(s, B, G))) return rc;
-    IpmData *D = scpb_internal_cone_data(s->cone);
-    const ConeSymbolic *S = scpb_internal_cone_sym(s->cone);
-    const IpmOpts o = scpb_internal_make_opts(opts);
-    cudaStream_t st = h->stream;
-    const size_t nX = (size_t)B * d.N * d.nx, nU = (size_t)B * d.N * d.nu, nP = (size_t)B * d.np;
-    SCPB_CUDA(h, cudaMemcpyAsync(s->xd, xd0, sizeof(double) * nX, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->ud, ud0, sizeof(double) * nU, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->p, p0, sizeof(double) * nP, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->src, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->src2, 0, sizeof(double) * (size_t)d.nsrc * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->done, 0, sizeof(int) * s->capB, st));
-    SCPB_CUDA(h, cudaMemsetAsync(s->iters, 0, sizeof(int) * s->capB, st));
-    std::vector<int> init_status(s->capB, 1);
-    SCPB_CUDA(h, cudaMemcpyAsync(s->status, init_status.data(), sizeof(int) * s->capB, cudaMemcpyHostToDevice, st));
-    std::vector<double> nanv(s->capB, nan(""));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->devi, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->J_out, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));
-    SCPB_CUDA(h, cudaMemcpyAsync(s->J_ref, nanv.data(), sizeof(double) * s->capB, cudaMemcpyHostToDevice, st));  // the guess has no J_aug
-    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->eta, v.eta_init, s->capB);
-    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->lam, v.lam_init, s->capB);
+    scpb_handle_s *h = s->h;
+    const scpb_ptr_desc &d = s->d;
+    const scpb_gusto_desc &g = s->gv;
+    cudaStream_t st = v.st;
+    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->eta, g.eta_init, s->capB);
+    k_fill<<<(s->capB + 127) / 128, 128, 0, st>>>(s->lam, g.lam_init, s->capB);
     h->launches += 2;
-
-    const size_t nsc = (size_t)(d.nx + d.nu + d.np);
-    const double *Sx = s->scale, *Su = Sx + d.nx, *Sp = Su + d.nu, *cx = s->scale + nsc, *cu = cx + d.nx, *cp = cu + d.nu;
-    PtrDev pd{};
-    pd.B = B; pd.G = G; pd.N = d.N; pd.nx = d.nx; pd.nu = d.nu; pd.np = d.np; pd.ns = d.ns;
-    pd.nsrc = d.nsrc; pd.oC = d.oC; pd.oD = d.oD; pd.oG = d.oG; pd.ors = d.ors; pd.oxh = d.oxh; pd.ouh = d.ouh; pd.oph = d.oph;
-    pd.t_grid = s->tgrid; pd.Sx = Sx; pd.cx = cx; pd.Su = Su; pd.cu = cu; pd.Sp = Sp; pd.cp = cp;
-    pd.src = s->src; pd.par = s->par; pd.eta = s->eta; pd.oeta = v.oeta; pd.lam = s->lam; pd.olam = v.olam;
-    AsmDev ad{};
-    ad.B = B; ad.G = G; ad.nsrc = d.nsrc; ad.nval = d.nval; ad.nnzA = (int)S->A_ci.size(); ad.nnzG = (int)S->G_ci.size();
-    ad.n = S->n; ad.p = S->p; ad.m = S->m; ad.W_rp = s->W_rp; ad.W_ci = s->W_ci; ad.W_v = s->W_v; ad.src = s->src;
-    ad.Av = D->Av; ad.Gv = D->Gv; ad.c = D->c; ad.b = D->b; ad.h = D->h; ad.c0 = s->c0;
-    StepDev sd{};   // k_extract only: J_new = pobj + c0 is the subproblem's L_aug
-    sd.B = B; sd.G = G; sd.N = d.N; sd.nx = d.nx; sd.nu = d.nu; sd.np = d.np; sd.n = S->n; sd.vx = d.vx; sd.vu = d.vu; sd.vp = d.vp;
-    sd.q_exit = d.q_exit; sd.eps_abs = d.eps_abs; sd.eps_rel = d.eps_rel;
-    sd.Sx = Sx; sd.cx = cx; sd.Su = Su; sd.cu = cu; sd.Sp = Sp; sd.cp = cp;
-    sd.xsol = D->x; sd.pobj = D->pobj; sd.c0 = s->c0; sd.cone_status = D->status;
-    sd.xd = s->xd; sd.ud = s->ud; sd.p = s->p; sd.xn = s->xn; sd.un = s->un; sd.pn = s->pn;
-    sd.J_ref = s->J_ref; sd.J_new = s->J_new; sd.dev = s->devi; sd.imp = s->imp; sd.feas_new = s->feas;
-    sd.done = s->done; sd.status = s->status; sd.iters = s->iters; sd.nactive = s->nactive;
+    v.pd.eta = s->eta; v.pd.oeta = g.oeta; v.pd.lam = s->lam; v.pd.olam = g.olam;
+    const StepDev &sd = v.sd;   // its J_new = pobj + c0 is the subproblem's L_aug
     GustoDev gd{};
-    gd.B = B; gd.G = G; gd.N = d.N; gd.nx = d.nx; gd.nu = d.nu; gd.np = d.np; gd.n = S->n; gd.vx = d.vx; gd.vu = d.vu; gd.vp = d.vp;
-    gd.q_exit = d.q_exit; gd.q_tr = v.q_tr; gd.iter_max = d.iter_max; gd.iter_mu = v.iter_mu; gd.nsq = v.nsq;
-    gd.lam_init = v.lam_init; gd.lam_max = v.lam_max; gd.rho_0 = v.rho_0; gd.rho_1 = v.rho_1; gd.beta_sh = v.beta_sh;
-    gd.beta_gr = v.beta_gr; gd.gamma_fail = v.gamma_fail; gd.eta_lb = v.eta_lb; gd.eta_ub = v.eta_ub; gd.mu = v.mu;
+    gd.B = B; gd.G = v.G; gd.N = d.N; gd.nx = d.nx; gd.nu = d.nu; gd.np = d.np; gd.n = sd.n; gd.vx = d.vx; gd.vu = d.vu; gd.vp = d.vp;
+    gd.q_exit = d.q_exit; gd.q_tr = g.q_tr; gd.iter_max = d.iter_max; gd.iter_mu = g.iter_mu; gd.nsq = g.nsq;
+    gd.lam_init = g.lam_init; gd.lam_max = g.lam_max; gd.rho_0 = g.rho_0; gd.rho_1 = g.rho_1; gd.beta_sh = g.beta_sh;
+    gd.beta_gr = g.beta_gr; gd.gamma_fail = g.gamma_fail; gd.eta_lb = g.eta_lb; gd.eta_ub = g.eta_ub; gd.mu = g.mu;
     gd.eps_abs = d.eps_abs; gd.eps_rel = d.eps_rel;
     gd.Q_rp = s->Q_rp; gd.Q_ci = s->Q_ci; gd.Q_v = s->Q_v; gd.Q_c = s->Q_c; gd.Q_w = s->Q_w;
-    gd.Sx = Sx; gd.cx = cx; gd.Su = Su; gd.cu = cu; gd.Sp = Sp; gd.cp = cp; gd.t_grid = s->tgrid; gd.xsol = D->x;
-    gd.par = s->par;
+    gd.Sx = sd.Sx; gd.cx = sd.cx; gd.Su = sd.Su; gd.cu = sd.cu; gd.Sp = sd.Sp; gd.cp = sd.cp; gd.t_grid = s->tgrid;
+    gd.xsol = v.D->x; gd.par = s->par;
     gd.xd = s->xd; gd.ud = s->ud; gd.p = s->p; gd.xn = s->xn; gd.un = s->un; gd.pn = s->pn;
     gd.J_ref = s->J_ref; gd.L_aug = s->J_new; gd.J_out = s->J_out; gd.eta = s->eta; gd.lam = s->lam; gd.dev = s->devi;
     gd.nodeq = s->nodeq; gd.nodef = s->nodef;
-    gd.cone_status = D->status; gd.feas_new = s->feas;
+    gd.cone_status = v.D->status; gd.feas_new = s->feas;
     gd.done = s->done; gd.status = s->status; gd.iters = s->iters; gd.nactive = s->nactive; gd.accept = s->accept;
-    ScvxDev cv{};   // k_scvx_take_dltv only
-    cv.B = B; cv.G = G; cv.nsrc = d.nsrc; cv.dltv_lo = d.oA; cv.dltv_hi = d.oC; cv.accept = s->accept; cv.src = s->src; cv.src2 = s->src2;
-
-    EventList evl;
-    std::vector<cudaEvent_t> &ev = evl.ev;
-    auto mark = [&]() { cudaEvent_t e; cudaEventCreate(&e); cudaEventRecord(e, st); ev.push_back(e); };
-    std::vector<int> phase;
-    mark(); phase.push_back(-1);
-    if ((rc = run_discretize(s, B, G, s->xd, s->ud, s->p))) return rc;   // generate_initial_guess -> discretize! (gusto.jl:517-526)
-    mark(); phase.push_back(0);
-    const int nbn = (int)(((long long)B * d.N + 127) / 128);
-    const int Bpad = s->capB;
-    int it = 1, nact = B, total_it = 0;
-    long long ipm_iters = 0;
-    std::vector<int> hit(B), hdone(B, 0);   // hdone: seeds that were already finished when the solver was launched (skipped)
-    const long long span = (long long)(d.oC - d.oA) * B;
-    for (; it <= d.iter_max; it++) {
-        launch_linearize(s, pd, nbn, st);
-        const long long tot = (long long)d.nval * Bpad;
-        k_assemble<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(ad);
-        h->launches += 2;
-        mark(); phase.push_back(1);
-        if ((rc = scpb_internal_cone_run(s->cone, o, s->done, nullptr, 0, 0))) return rc;
-        mark(); phase.push_back(2);
-        SCPB_CUDA(h, cudaMemcpyAsync(hit.data(), D->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        sd.iter = it;
-        k_extract<<<nbn, 128, 0, st>>>(sd);
-        h->launches++;
-        mark(); phase.push_back(3);
-        if ((rc = run_discretize(s, B, G, s->xn, s->un, s->pn, s->src2, s->done))) return rc;   // candidate: DLTV into src2
-        mark(); phase.push_back(0);
-        SCPB_CUDA(h, cudaMemsetAsync(s->nactive, 0, sizeof(int), st));
+    v.opts_at = [&](int) { return v.o; };
+    v.cand_src = s->src2;
+    v.step = [&](int it, cudaStream_t, int) -> int {
         gd.iter = it;
-        if (launch_gusto_nodes(s, gd, st)) return set_err(h, SCPB_ERR_UNSUPPORTED, "gusto_solve: no device pack for model %d", s->model_id);
+        if (launch_gusto_nodes(s, gd, st))
+            return set_err(h, SCPB_ERR_UNSUPPORTED, "gusto_solve: no device pack for model %d", s->model_id);
         k_gusto_step<<<(B + 63) / 64, 64, 0, st>>>(gd);
-        k_scvx_take_dltv<<<(unsigned)((span + 255) / 256), 256, 0, st>>>(cv);
+        take_dltv(v);
         h->launches += 3;
-        SCPB_CUDA(h, cudaMemcpyAsync(&nact, s->nactive, sizeof(int), cudaMemcpyDeviceToHost, st));
-        mark(); phase.push_back(3);
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        for (int b = 0; b < B; b++) if (!hdone[b]) ipm_iters += hit[b];   // skipped seeds keep a stale count in D->iters
-        ipm_launch_stats(hit, hdone, total_it + 1);
-        SCPB_CUDA(h, cudaMemcpyAsync(hdone.data(), s->done, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-        SCPB_CUDA(h, cudaStreamSynchronize(st));
-        total_it++;
-        if (nact == 0) break;
-    }
-    SCPB_CUDA(h, cudaGetLastError());
-    if (xd) SCPB_CUDA(h, cudaMemcpyAsync(xd, s->xd, sizeof(double) * nX, cudaMemcpyDeviceToHost, st));
-    if (ud) SCPB_CUDA(h, cudaMemcpyAsync(ud, s->ud, sizeof(double) * nU, cudaMemcpyDeviceToHost, st));
-    if (p) SCPB_CUDA(h, cudaMemcpyAsync(p, s->p, sizeof(double) * nP, cudaMemcpyDeviceToHost, st));
-    if (status) SCPB_CUDA(h, cudaMemcpyAsync(status, s->status, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (iters) SCPB_CUDA(h, cudaMemcpyAsync(iters, s->iters, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (J) SCPB_CUDA(h, cudaMemcpyAsync(J, s->J_out, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (deviation) SCPB_CUDA(h, cudaMemcpyAsync(deviation, s->devi, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (feas) SCPB_CUDA(h, cudaMemcpyAsync(feas, s->feas, sizeof(int) * B, cudaMemcpyDeviceToHost, st));
-    if (eta) SCPB_CUDA(h, cudaMemcpyAsync(eta, s->eta, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    if (lam) SCPB_CUDA(h, cudaMemcpyAsync(lam, s->lam, sizeof(double) * B, cudaMemcpyDeviceToHost, st));
-    SCPB_CUDA(h, cudaStreamSynchronize(st));
-    double acc[4] = {0, 0, 0, 0};
-    for (size_t i = 1; i < ev.size(); i++) {
-        float ms = 0.f;
-        cudaEventElapsedTime(&ms, ev[i - 1], ev[i]);
-        if (phase[i] >= 0) acc[phase[i]] += ms * 1e-3;
-    }
-    float tot_ms = 0.f;
-    cudaEventElapsedTime(&tot_ms, ev.front(), ev.back());
-    if (timing) {
-        timing[0] = acc[0]; timing[1] = acc[1]; timing[2] = acc[2]; timing[3] = acc[3];
-        timing[4] = tot_ms * 1e-3; timing[5] = (double)total_it; timing[6] = (double)ipm_iters; timing[7] = 0.0;
-    }
-    return ptr_check_disc_status(h, "gusto_solve");
+        return SCPB_OK;
+    };
+
+    v.mark(-1, st);
+    if ((rc = run_discretize(s, B, v.G, s->xd, s->ud, s->p))) return rc;   // generate_initial_guess -> discretize! (gusto.jl:517-526)
+    v.mark(0, st);
+    if ((rc = lockstep_loop(v, d.iter_max))) return rc;
+    return solve_end(v, xd, ud, p, status, iters, J, s->J_out, deviation, feas, {{eta, s->eta}, {lam, s->lam}}, timing, 8,
+                     "gusto_solve");
 }
 
 }  // extern "C"

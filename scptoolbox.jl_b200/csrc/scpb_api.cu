@@ -54,15 +54,8 @@ int scpb_internal_discretize(scpb_handle_s *h, DiscArgs &a, double feas_tol, int
     double *dn = (double *)h->scratch(0, sizeof(double) * (size_t)a.B * (a.N - 1));
     if (!dn) return set_err(h, SCPB_ERR_CUDA, "scratch allocation failed");
     a.dnorm = dn;
-    switch (h->model_id) {
-    case SCPB_MODEL_DBLINT: rc = launch_disc<Model<SCPB_MODEL_DBLINT>>(h, a, method, st); break;
-    case SCPB_MODEL_ROCKET: rc = launch_disc<Model<SCPB_MODEL_ROCKET>>(h, a, method, st); break;
-    case SCPB_MODEL_STARSHIP: rc = launch_disc<Model<SCPB_MODEL_STARSHIP>>(h, a, method, st); break;
-    case SCPB_MODEL_QUADROTOR: rc = launch_disc<Model<SCPB_MODEL_QUADROTOR>>(h, a, method, st); break;
-    case SCPB_MODEL_FREEFLYER: rc = launch_disc<Model<SCPB_MODEL_FREEFLYER>>(h, a, method, st); break;
-    case SCPB_MODEL_RENDEZVOUS2D: rc = launch_disc<Model<SCPB_MODEL_RENDEZVOUS2D>>(h, a, method, st); break;
-    default: return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", h->model_id);
-    }
+    if (!with_model(h->model_id, [&](auto m) { rc = launch_disc<decltype(m)>(h, a, method, st); }))
+        return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", h->model_id);
     if (rc) return rc;
     if (feas) {
         const int cnt = a.nb > 0 ? a.nb : a.B;
@@ -157,16 +150,9 @@ int32_t scpb_model_set(scpb_handle h, int32_t model_id, const double *par, int32
 {
     if (!h) return SCPB_ERR_ARG;
     if (npar < 0 || npar > SCPB_MAX_PAR || (npar > 0 && !par)) return set_err(h, SCPB_ERR_ARG, "bad parameter block");
-    int enx = 0, enu = 0, enp_min = 1;
-    switch (model_id) {
-    case SCPB_MODEL_DBLINT: enx = 2; enu = 1; break;
-    case SCPB_MODEL_ROCKET: enx = 7; enu = 4; break;
-    case SCPB_MODEL_STARSHIP: enx = 8; enu = 3; enp_min = 2; break;
-    case SCPB_MODEL_QUADROTOR: enx = 6; enu = 4; break;
-    case SCPB_MODEL_FREEFLYER: enx = 13; enu = 6; break;
-    case SCPB_MODEL_RENDEZVOUS2D: enx = 6; enu = 12; break;
-    default: return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", model_id);
-    }
+    int enx = 0, enu = 0, enp_min = 0;   // np >= the leading parameters the dynamics pack reads
+    if (!with_model(model_id, [&](auto m) { enx = decltype(m)::NX; enu = decltype(m)::NU; enp_min = decltype(m)::NPD; }))
+        return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", model_id);
     if (nx != enx || nu != enu || np < enp_min)
         return set_err(h, SCPB_ERR_MODEL, "model %d expects nx=%d nu=%d np>=%d, got %d %d %d", model_id, enx, enu,
                        enp_min, nx, nu, np);
@@ -351,15 +337,8 @@ int32_t scpb_propagate(scpb_handle h, int32_t method, int32_t B, int32_t N, int3
     a.par = h->par;
     cudaEvent_t e0 = h->ev0, e1 = h->ev1;   // the handle's own pair: nothing to leak on an error path
     SCPB_CUDA(h, cudaEventRecord(e0, st));
-    switch (h->model_id) {
-    case SCPB_MODEL_DBLINT: rc = launch_prop<Model<SCPB_MODEL_DBLINT>>(h, a, method, subres); break;
-    case SCPB_MODEL_ROCKET: rc = launch_prop<Model<SCPB_MODEL_ROCKET>>(h, a, method, subres); break;
-    case SCPB_MODEL_STARSHIP: rc = launch_prop<Model<SCPB_MODEL_STARSHIP>>(h, a, method, subres); break;
-    case SCPB_MODEL_QUADROTOR: rc = launch_prop<Model<SCPB_MODEL_QUADROTOR>>(h, a, method, subres); break;
-    case SCPB_MODEL_FREEFLYER: rc = launch_prop<Model<SCPB_MODEL_FREEFLYER>>(h, a, method, subres); break;
-    case SCPB_MODEL_RENDEZVOUS2D: rc = launch_prop<Model<SCPB_MODEL_RENDEZVOUS2D>>(h, a, method, subres); break;
-    default: return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", h->model_id);
-    }
+    if (!with_model(h->model_id, [&](auto m) { rc = launch_prop<decltype(m)>(h, a, method, subres); }))
+        return set_err(h, SCPB_ERR_MODEL, "unknown model id %d", h->model_id);
     if (rc) return rc;
     SCPB_CUDA(h, cudaEventRecord(e1, st));
     SCPB_CUDA(h, cudaGetLastError());

@@ -31,7 +31,7 @@ import numpy as np
 
 from . import lib
 from .parser import ConicTemplate, Expr, Lin, matvec
-from .ptr import FOH, SCPBatchSolution, SCPProblem, SourceMap, trapz  # noqa: F401
+from .ptr import FOH, SCPBatchSolution, SCPProblem, SourceMap, guess_arrays, run_solve, trapz  # noqa: F401
 from .scvx import _rows_matrix
 
 
@@ -212,43 +212,11 @@ def solve(pbm: GuSTOProblem, guesses=None, project_guess=True, **cone_opts) -> S
     generate_initial_guess (gusto.jl:517-526) the guesses are first projected onto the convex path constraints
     (correct_convex!, scp.jl:275-361) -- one batched call of the GPU cone solver."""
     from .ptr import correct_convex
-    traj, pars, h = pbm.traj, pbm.pars, pbm.handle
-    if guesses is None:
-        x0, u0, p0 = traj.guess(pars.N)
-        guesses = (x0[None], u0[None], p0[None])
-    if hasattr(guesses, "xd") and hasattr(guesses, "ud"):      # warm start from an earlier batch solution (solve(pbm, warm),
-        guesses = (guesses.xd, guesses.ud, guesses.p)           # scp.jl:532-539: its discrete trajectory is the initial guess)
-        project_guess = False                                   # gusto.jl:434-438: a warm start is not re-projected
-    xd0 = np.ascontiguousarray(guesses[0], dtype=np.float64)
-    ud0 = np.ascontiguousarray(guesses[1], dtype=np.float64)
-    p0 = np.ascontiguousarray(guesses[2], dtype=np.float64)
+    if hasattr(guesses, "xd") and hasattr(guesses, "ud"):      # a warm start from an earlier batch solution
+        project_guess = False                                   # gusto.jl:434-438: is not re-projected
+    g = guess_arrays(pbm, guesses)
     if project_guess:
-        xd0, ud0, p0 = correct_convex(pbm, (xd0, ud0, p0))
-    B, N = xd0.shape[0], pars.N
-    assert xd0.shape == (B, N, traj.nx) and ud0.shape == (B, N, traj.nu) and p0.shape == (B, traj.np)
-    o = lib.ConeOpts()
-    o.nref = -1
-    o.equil = -1
-    if pars.solver_opts and "maxit" in pars.solver_opts:
-        o.maxit = int(pars.solver_opts["maxit"])
-    for k_, v in cone_opts.items():
-        setattr(o, k_, v)
-    xd, ud, p = np.empty_like(xd0), np.empty_like(ud0), np.empty_like(p0)
-    status = np.zeros(B, dtype=np.int32); iters = np.zeros(B, dtype=np.int32); feas = np.zeros(B, dtype=np.int32)
-    J = np.empty(B); dev = np.empty(B); eta = np.empty(B); lam = np.empty(B); timing = np.zeros(8)
-    dp = lambda a: a.ctypes.data_as(lib._dp)
-    ip = lambda a: a.ctypes.data_as(lib._ip)
-    rc = h.lib.scpb_gusto_solve(pbm.ptr, B, dp(xd0), dp(ud0), dp(p0), C.cast(C.byref(o), C.c_void_p), dp(xd), dp(ud),
-                                dp(p), ip(status), ip(iters), dp(J), dp(dev), ip(feas), dp(eta), dp(lam), dp(timing))
-    h._check(rc, "scpb_gusto_solve")
-    names = []
-    for s_ in status:
-        if s_ in (0, 1):
-            names.append("SCP_SOLVED")
-        else:
-            names.append(f"SCP_FAILED ({lib.CONE_STATUS.get((int(s_) - 2) // 16, '?')})")
-    tm = dict(discretize=timing[0], formulate=timing[1], solve=timing[2], overhead=timing[3], total=timing[4],
-              lockstep_iterations=int(timing[5]), ipm_iterations=int(timing[6]))
-    sol = SCPBatchSolution(names, iters, J, pbm.t, xd, ud, p, dev, feas, tm, status)
+        g = correct_convex(pbm, g)
+    sol, (eta, lam) = run_solve(pbm, pbm.handle.lib.scpb_gusto_solve, g, cone_opts, n_extra=2)
     sol.eta, sol.lam = eta, lam
     return sol

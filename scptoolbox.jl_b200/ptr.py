@@ -462,26 +462,29 @@ def set_homotopy(pbm: SCPProblem, B, beta=None):
     h._check(h.lib.scpb_ptr_set_homotopy_beta(pbm.ptr, B, pb), "scpb_ptr_set_homotopy_beta")
 
 
-def solve(pbm: SCPProblem, guesses=None, beta=None, **cone_opts) -> SCPBatchSolution:
-    """PTR.solve (ptr.jl:448-532) for a batch: guesses = (xd0 (B,N,nx), ud0 (B,N,nu), p0 (B,np));
-    None => the problem's own guess (one seed).  The model's parameter block is read again here, as the reference's
-    closures read the model at call time: a parameter changed between two solves (a homotopy step) takes effect
-    without a new create.
-    beta: update threshold of the problem's in-loop homotopy schedule, a scalar or one per seed (None: the one given to
-    problem_set_homotopy_update), so a sweep over thresholds is one batch."""
-    traj, pars, h = pbm.traj, pbm.pars, pbm.handle
-    set_parameters(pbm)
+def guess_arrays(pbm: SCPProblem, guesses):
+    """guesses = (xd0 (B,N,nx), ud0 (B,N,nu), p0 (B,np)), an earlier batch solution (a warm start, solve(pbm, warm),
+    scp.jl:532-539: its discrete trajectory is the initial guess) or None (the problem's own guess, one seed) ->
+    contiguous float64 arrays"""
+    traj, N = pbm.traj, pbm.pars.N
     if guesses is None:
-        x0, u0, p0 = traj.guess(pars.N)
+        x0, u0, p0 = traj.guess(N)
         guesses = (x0[None], u0[None], p0[None])
-    if hasattr(guesses, "xd") and hasattr(guesses, "ud"):      # warm start from an earlier batch solution (solve(pbm, warm),
-        guesses = (guesses.xd, guesses.ud, guesses.p)           # scp.jl:532-539: its discrete trajectory is the initial guess)
-    xd0 = np.ascontiguousarray(guesses[0], dtype=np.float64)
-    ud0 = np.ascontiguousarray(guesses[1], dtype=np.float64)
-    p0 = np.ascontiguousarray(guesses[2], dtype=np.float64)
-    B, N = xd0.shape[0], pars.N
+    if hasattr(guesses, "xd") and hasattr(guesses, "ud"):
+        guesses = (guesses.xd, guesses.ud, guesses.p)
+    xd0, ud0, p0 = (np.ascontiguousarray(g, dtype=np.float64) for g in guesses)
+    B = xd0.shape[0]
     assert xd0.shape == (B, N, traj.nx) and ud0.shape == (B, N, traj.nu) and p0.shape == (B, traj.np)
-    set_homotopy(pbm, B, beta)
+    return xd0, ud0, p0
+
+
+def run_solve(pbm: SCPProblem, fn, guesses, cone_opts, n_extra=0, n_timing=8):
+    """One call of the C solve fn (scpb_ptr_solve, scpb_scvx_solve or scpb_gusto_solve) on the guess arrays: the batch
+    solution and the n_extra per-seed outputs that follow feas (SCvx: eta; GuSTO: eta, lambda).  The cone options are
+    the reference's (nref = equil = -1, solver_opts["maxit"]) with the keyword arguments on top."""
+    h, pars = pbm.handle, pbm.pars
+    xd0, ud0, p0 = guesses
+    B = xd0.shape[0]
     o = lib.ConeOpts()
     o.nref = -1
     o.equil = -1
@@ -491,28 +494,43 @@ def solve(pbm: SCPProblem, guesses=None, beta=None, **cone_opts) -> SCPBatchSolu
         setattr(o, k_, v)
     xd, ud, p = np.empty_like(xd0), np.empty_like(ud0), np.empty_like(p0)
     status = np.zeros(B, dtype=np.int32); iters = np.zeros(B, dtype=np.int32); feas = np.zeros(B, dtype=np.int32)
-    J = np.empty(B); dev = np.empty(B); timing = np.zeros(10)
+    J = np.empty(B); dev = np.empty(B); extras = [np.empty(B) for _ in range(n_extra)]; timing = np.zeros(n_timing)
     dp = lambda a: a.ctypes.data_as(lib._dp)
     ip = lambda a: a.ctypes.data_as(lib._ip)
-    rc = h.lib.scpb_ptr_solve(pbm.ptr, B, dp(xd0), dp(ud0), dp(p0), C.cast(C.byref(o), C.c_void_p), dp(xd), dp(ud),
-                              dp(p), ip(status), ip(iters), dp(J), dp(dev), ip(feas), dp(timing))
-    h._check(rc, "scpb_ptr_solve")
-    names = []
-    for s_ in status:
-        if s_ in (0, 1):
-            names.append("SCP_SOLVED")     # scp.jl:221-222: anything but an unsafe solver status is reported solved
-        else:
-            names.append(f"SCP_FAILED ({lib.CONE_STATUS.get((int(s_) - 2) // 16, '?')})")
+    rc = fn(pbm.ptr, B, dp(xd0), dp(ud0), dp(p0), C.cast(C.byref(o), C.c_void_p), dp(xd), dp(ud), dp(p), ip(status),
+            ip(iters), dp(J), dp(dev), ip(feas), *[dp(e) for e in extras], dp(timing))
+    h._check(rc, fn.__name__)
+    # scp.jl:221-222: anything but an unsafe solver status is reported solved
+    names = ["SCP_SOLVED" if s_ in (0, 1) else f"SCP_FAILED ({lib.CONE_STATUS.get((int(s_) - 2) // 16, '?')})"
+             for s_ in status]
     tm = dict(discretize=timing[0], formulate=timing[1], solve=timing[2], overhead=timing[3], total=timing[4],
-              lockstep_iterations=int(timing[5]), ipm_iterations=int(timing[6]), chunks=int(timing[7]),
-              initial_discretize=timing[8])
-    sol = SCPBatchSolution(names, iters, J, pbm.t, xd, ud, p, dev, feas, tm, status)
+              lockstep_iterations=int(timing[5]), ipm_iterations=int(timing[6]))
+    if n_timing > 8:        # PTR: streamed chains and the initial discretize!
+        tm.update(chunks=int(timing[7]), initial_discretize=timing[8])
+    return SCPBatchSolution(names, iters, J, pbm.t, xd, ud, p, dev, feas, tm, status), extras
+
+
+def solve(pbm: SCPProblem, guesses=None, beta=None, **cone_opts) -> SCPBatchSolution:
+    """PTR.solve (ptr.jl:448-532) for a batch: guesses = (xd0 (B,N,nx), ud0 (B,N,nu), p0 (B,np));
+    None => the problem's own guess (one seed).  The model's parameter block is read again here, as the reference's
+    closures read the model at call time: a parameter changed between two solves (a homotopy step) takes effect
+    without a new create.
+    beta: update threshold of the problem's in-loop homotopy schedule, a scalar or one per seed (None: the one given to
+    problem_set_homotopy_update), so a sweep over thresholds is one batch."""
+    traj, pars, h = pbm.traj, pbm.pars, pbm.handle
+    set_parameters(pbm)
+    g = guess_arrays(pbm, guesses)
+    B = g[0].shape[0]
+    set_homotopy(pbm, B, beta)
+    sol, _ = run_solve(pbm, h.lib.scpb_ptr_solve, g, cone_opts, n_timing=10)
     sol.iter_max = np.full(B, pars.iter_max, dtype=np.int32)
     if getattr(traj, "hom", None) is not None:
         cap = homotopy_history_length(pbm)
         sol.hom_index = np.zeros(B, dtype=np.int32)
         hidx, himp = np.zeros((B, cap), dtype=np.int32), np.zeros((B, cap))
-        rc = h.lib.scpb_ptr_homotopy_result(pbm.ptr, B, ip(sol.hom_index), ip(sol.iter_max), cap, ip(hidx), dp(himp))
+        ip = lambda a: a.ctypes.data_as(lib._ip)
+        rc = h.lib.scpb_ptr_homotopy_result(pbm.ptr, B, ip(sol.hom_index), ip(sol.iter_max), cap, ip(hidx),
+                                            himp.ctypes.data_as(lib._dp))
         h._check(rc, "scpb_ptr_homotopy_result")
         sol.hom_history = {"index": hidx, "improv_rel": himp}
     return sol

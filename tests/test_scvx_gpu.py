@@ -87,3 +87,16 @@ def test_scvx_first_iterations_are_identical(pkg, handle):
     dJ = abs(sol.cost[0] - rs.J_aug) / max(1.0, abs(rs.J_aug))
     print("scvx 3 iterations: ex(phys)", ex7, "dJ", dJ, "J", sol.cost[0], rs.J_aug)
     assert dJ <= 1e-7 and ex7 <= 1e-7
+
+
+def test_scvx_refuses_a_constraint_pack_it_has_no_penalty_for(pkg, handle):
+    """The nonlinear cost of SCvx has the nonconvex-constraint penalty of the starship's pack only: a problem with
+    another pack (the quadrotor's obstacles) is refused when SCvx is attached, not solved without its penalty."""
+    ex = pkg.examples.quadrotor
+    traj = pkg.problem.TrajectoryProblem(ex.QuadrotorProblem())
+    ex.define_problem(traj, "scvx", handle=handle)
+    assert traj.ns > 0
+    pars = pkg.scvx.Parameters(N=10, Nsub=15, iter_max=5, disc_method=pkg.ptr.FOH, q_tr=np.inf, q_exit=np.inf,
+                               solver_opts={"verbose": 0}, **KW)
+    with pytest.raises(pkg.lib.ScpbError, match=r"scpb_scvx_attach failed \(-4\).*no penalty for the constraint pack"):
+        pkg.scvx.create(pars, traj, handle)
