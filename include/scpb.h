@@ -34,11 +34,15 @@ enum {
                                  par: m, J, lcg, lcp, CD, alpha_e, rate_delay, g0, tau_s           */
     SCPB_MODEL_QUADROTOR = 4, /* quadrotor/definition.jl:140-186; par: g[3]                        */
     SCPB_MODEL_FREEFLYER = 5, /* freeflyer/definition.jl:224-284; par: mass, J[9], Jinv[9] (col-major) */
-    SCPB_MODEL_RENDEZVOUS2D = 6 /* rendezvous_planar/definition.jl:147-243 (impulsive RCS thrust): x=[r2,v2,theta,omega],
+    SCPB_MODEL_RENDEZVOUS2D = 6, /* rendezvous_planar/definition.jl:147-243 (impulsive RCS thrust): x=[r2,v2,theta,omega],
                                  u[0..2]=(f-,f+,f0) of 12 inputs, p=[tdil]; par: m, J, lu, lv, n.  The only pack with
                                  impulse semantics (the reference's f/B called with a negative segment index).
                                  Its constraint pack (the RCS deadband, definition.jl:337-413: ns = 6, ng = 1) reads
                                  par[5] = f_db, par[6] = f_max, par[7] = kappa, the sharpness of the smooth OR */
+    SCPB_MODEL_OSCILLATOR = 7 /* oscillator/definition.jl:161-236 (fixed final time: F = 0, no time-dilation column):
+                                 x=[r,v], u=[aa,ar,l1aa,l1adiff], p=[l1r_1..l1r_N] (np must be N); par: zeta, omega0, tf.
+                                 Its constraint pack (the input deadband, definition.jl:370-444: ns = 2, ng = 1, the
+                                 node's own parameter) reads par[3] = a_db, par[4] = a_max, par[5] = kappa */
 };
 #define SCPB_MAX_PAR 64
 
@@ -164,6 +168,7 @@ int32_t scpb_cone_solve(scpb_cone c, int32_t B, const double *Avals, const doubl
  * the fill matrix W with [Avals; Gvals; c; b; h; c0] = W * src, where src is the per-seed vector of
  * device-computed quantities laid out by the offsets below (source 0 is the constant 1):
  *   oA,oBm,oBp,oF,or_,oE : DLTV blocks per segment (column-major nx*nx, nx*nu, nx*nf, nx) -- discretize!
+ *                          (nf = 0 for a model with a fixed final time: the F block is empty)
  *   oC,oD,oG,ors         : ds/dx, ds/du, ds/dp (row-major; ds/dp packed to ng columns, see csrc/constraints.cuh)
  *                          and r = s - Cx - Du - Gp per node (scp.jl:763-773)
  *   oxh,ouh,oph          : scaled reference trajectory (ptr.jl:575-577)

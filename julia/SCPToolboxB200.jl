@@ -6,6 +6,10 @@ module SCPToolboxB200
 
 const libscpb = joinpath(@__DIR__, "..", "scptoolbox.jl_b200", "libscpb.so")
 
+# device model packs, the `id` of model_set! (SCPB_MODEL_*, include/scpb.h)
+const MODEL_DBLINT, MODEL_ROCKET, MODEL_STARSHIP, MODEL_QUADROTOR, MODEL_FREEFLYER, MODEL_RENDEZVOUS2D = 1, 2, 3, 4, 5, 6
+const MODEL_OSCILLATOR = 7    # fixed final time (no F column); np = N, one l1r slack per node
+
 mutable struct Handle
     ptr::Ptr{Cvoid}
 end

@@ -11,4 +11,5 @@ from .examples import double_integrator as _double_integrator  # noqa: F401
 from .examples import freeflyer as _freeflyer  # noqa: F401
 from .examples import quadrotor as _quadrotor  # noqa: F401
 from .examples import rendezvous_planar as _rendezvous_planar  # noqa: F401
+from .examples import oscillator as _oscillator  # noqa: F401
 from .lib import Handle, ScpbError  # noqa: F401

@@ -153,13 +153,70 @@ struct Constr<SCPB_MODEL_FREEFLYER> {
     }
 };
 
+// Smooth logical OR of scalar predicates with scalar gradients, the reference's
+//   or(pred, grad; kappa, match, normalize) -> indicator -> sigmoid -> logsumexp   (src/utils/helper.jl:623-807).
+// The predicates, their gradients and `match` are divided by `normalize`; the indicator shifts the sigmoid by
+// 1 - sigmoid(match) so that the OR is exact at the predicates' values `match` (one value or one per predicate).  Every
+// step keeps the reference's operation order, with no contraction into fma: at the sharp end of a homotopy
+// sigma = 1 - 1/(1 + exp(kappa L)) rounds to exactly 1 and the gradient factor c = exp(kappa L + 2 log(1 - sigma)) to
+// exactly 0, and a rearranged formula would not saturate on the same inputs.  The shift depends on kappa only, so it is
+// computed once per (seed, node) by the constructor.
+template <int NM>
+struct SmoothOr {
+    double kap, nrm, shift;
+    // sigmoid(f[, g]; kappa) of n predicates: the value, and with g its gradient *dsg
+    template <int n>
+    __device__ __forceinline__ static double sigmoid(const double (&f)[n], const double *g, double kap, double *dsg)
+    {
+        double a = __dmul_rn(kap, f[0]);
+#pragma unroll
+        for (int i = 1; i < n; i++) a = fmax(a, __dmul_rn(kap, f[i]));
+        double e[n], E = 0.0;
+#pragma unroll
+        for (int i = 0; i < n; i++) {
+            e[i] = exp(__dsub_rn(__dmul_rn(kap, f[i]), a));
+            E = i == 0 ? e[0] : __dadd_rn(E, e[i]);
+        }
+        const double L = __ddiv_rn(__dadd_rn(a, log(E)), kap);
+        const double kL = __dmul_rn(kap, L);
+        const double sg = __dsub_rn(1.0, __ddiv_rn(1.0, __dadd_rn(1.0, exp(kL))));
+        if (g) {
+            double dL = 0.0;
+#pragma unroll
+            for (int i = 0; i < n; i++) {
+                const double t = __dmul_rn(g[i], __ddiv_rn(e[i], E));
+                dL = i == 0 ? t : __dadd_rn(dL, t);
+            }
+            const double c = exp(__dadd_rn(kL, __dmul_rn(2.0, log(__dsub_rn(1.0, sg)))));
+            *dsg = __dmul_rn(__dmul_rn(kap, c), dL);
+        }
+        return sg;
+    }
+    __device__ __forceinline__ SmoothOr(double kappa, double normalize, const double (&match)[NM])
+        : kap(kappa), nrm(normalize)
+    {
+        double m[NM];
+#pragma unroll
+        for (int i = 0; i < NM; i++) m[i] = __ddiv_rn(match[i], nrm);
+        shift = __dsub_rn(1.0, sigmoid(m, nullptr, kap, nullptr));
+    }
+    // OR and dOR of the predicates pred with gradients grad (both before normalisation)
+    template <int NP>
+    __device__ __forceinline__ void operator()(const double (&pred)[NP], const double (&grad)[NP], double &OR,
+                                               double &dOR) const
+    {
+        double f[NP], g[NP];
+#pragma unroll
+        for (int i = 0; i < NP; i++) { f[i] = __ddiv_rn(pred[i], nrm); g[i] = __ddiv_rn(grad[i], nrm); }
+        OR = __dadd_rn(sigmoid(f, g, kap, &dOR), shift);
+    }
+};
+
 // rendezvous_planar/definition.jl:337-413: the RCS deadband.  For thruster i, with the smooth OR of the predicates
 // "reference thrust above / below the deadband",
-//   s_2i = f_i - OR(fr_i) fr_i,   s_2i+1 = OR(fr_i) fr_i - f_i,   D = +-1 on f_i, -+(dOR/dfr fr_i + OR) on fr_i.
-// OR = or(...; kappa, match, normalize) -> indicator -> sigmoid -> logsumexp (src/utils/helper.jl:623-807).  Every step
-// keeps the reference's operation order, with no contraction into fma: at the sharp end of the homotopy
-// (kappa ~ 4.6e3) sigma = 1 - 1/(1 + exp(kappa L)) rounds to exactly 1 and the gradient factor
-// c = exp(kappa L + 2 log(1 - sigma)) to exactly 0, and a rearranged formula would not saturate on the same inputs.
+//   s_2i = f_i - OR(fr_i) fr_i,   s_2i+1 = OR(fr_i) fr_i - f_i,   D = +-1 on f_i, -+(dOR/dfr fr_i + OR) on fr_i,
+// OR = or([fr - f_db, -f_db - fr], [1, -1]; kappa, match = [f_max - f_db, -f_db - f_max], normalize = f_max + f_db).
+// At the sharp end of the homotopy (kappa ~ 4.6e3) it saturates exactly (SmoothOr).
 // par: m, J, lu, lv, n (dynamics pack) [0..4], then f_db [5], f_max [6], kappa [7].
 // KAPPA names the slot of the homotopy parameter: eval_kappa takes kappa as an argument, so the PTR loop can pass each
 // seed's own value of an in-loop homotopy schedule (scpb_ptr_set_homotopy) without copying the parameter block.
@@ -167,20 +224,6 @@ template <>
 struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
     static constexpr int NS = 6, NX = 6, NU = 12, NG = 1, KAPPA = 7;
     __device__ static constexpr int gcol(int, int j) { return j; }
-    // sigmoid([f0, f1], [g0, g1]; kappa) of two scalar predicates with scalar gradients: value sg, gradient dsg
-    __device__ __forceinline__ static void sigmoid2(double f0, double f1, double g0, double g1, double kap, double &sg,
-                                                    double &dsg)
-    {
-        const double a = fmax(__dmul_rn(kap, f0), __dmul_rn(kap, f1));
-        const double e0 = exp(__dsub_rn(__dmul_rn(kap, f0), a)), e1 = exp(__dsub_rn(__dmul_rn(kap, f1), a));
-        const double E = __dadd_rn(e0, e1);
-        const double L = __ddiv_rn(__dadd_rn(a, log(E)), kap);
-        const double kL = __dmul_rn(kap, L);
-        sg = __dsub_rn(1.0, __ddiv_rn(1.0, __dadd_rn(1.0, exp(kL))));
-        const double dL = __dadd_rn(__dmul_rn(g0, __ddiv_rn(e0, E)), __dmul_rn(g1, __ddiv_rn(e1, E)));
-        const double c = exp(__dadd_rn(kL, __dmul_rn(2.0, log(__dsub_rn(1.0, sg)))));
-        dsg = __dmul_rn(__dmul_rn(kap, c), dL);
-    }
     __device__ static void eval(const ModelPar &P, double t, int N, int k, const double *x, const double *u,
                                 const double *p, double *s, double *C, double *D, double *G)
     {
@@ -190,19 +233,15 @@ struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
                                       const double *, double *s, double *C, double *D, double *G)
     {
         const double fdb = P.v[5], fmx = P.v[6];
-        const double nrm = __dadd_rn(fmx, fdb);
+        const SmoothOr<2> smooth_or(kap, __dadd_rn(fmx, fdb), {__dsub_rn(fmx, fdb), __dsub_rn(-fdb, fmx)});
         for (int i = 0; i < NS * NX; i++) C[i] = 0.0;
         for (int i = 0; i < NS * NU; i++) D[i] = 0.0;
         for (int i = 0; i < NS * NG; i++) G[i] = 0.0;
-        double off, unused;   // indicator's y-shift: the OR is exact at the predicates' values `match`
-        sigmoid2(__ddiv_rn(__dsub_rn(fmx, fdb), nrm), __ddiv_rn(__dsub_rn(-fdb, fmx), nrm), 0.0, 0.0, kap, off, unused);
-        const double shift = __dsub_rn(1.0, off);
         for (int i = 0; i < 3; i++) {
             const double f = u[i], fr = u[3 + i];
-            double sg, dOR;
-            sigmoid2(__ddiv_rn(__dsub_rn(fr, fdb), nrm), __ddiv_rn(__dsub_rn(-fdb, fr), nrm), __ddiv_rn(1.0, nrm),
-                     __ddiv_rn(-1.0, nrm), kap, sg, dOR);
-            const double OR = __dadd_rn(sg, shift), ORfr = __dmul_rn(OR, fr);
+            double OR, dOR;
+            smooth_or({__dsub_rn(fr, fdb), __dsub_rn(-fdb, fr)}, {1.0, -1.0}, OR, dOR);
+            const double ORfr = __dmul_rn(OR, fr);
             const double dORfr = __dadd_rn(__dmul_rn(dOR, fr), OR);
             s[2 * i] = __dsub_rn(f, ORfr);
             s[2 * i + 1] = __dsub_rn(ORfr, f);
@@ -211,5 +250,44 @@ struct Constr<SCPB_MODEL_RENDEZVOUS2D> {
             D[(2 * i + 1) * NU + i] = -1.0;
             D[(2 * i + 1) * NU + 3 + i] = dORfr;
         }
+    }
+};
+
+// oscillator/definition.jl:370-444: the input deadband.  With the smooth OR of the predicates "reference acceleration
+// above / below the deadband",
+//   s_0 = aa - OR(ar) ar,   s_1 = OR(ar) ar - aa,   D = +-1 on aa, -+(dOR/dar ar + OR) on ar,
+// OR = or([ar - a_db, -a_db - ar], [1, -1]; kappa, match = a_max - a_db, normalize = a_max - a_db): a SCALAR match, so
+// the indicator's shift is the sigmoid of one value (logsumexp of a single term).  C and G are zero; G is packed to the
+// node's own parameter l1r_k (NG = 1), which s does not read.
+// par: zeta, omega0, tf (dynamics pack) [0..2], then a_db [3], a_max [4], kappa [5] (KAPPA, as for the rendezvous).
+template <>
+struct Constr<SCPB_MODEL_OSCILLATOR> {
+    static constexpr int NS = 2, NX = 2, NU = 4, NG = 1, KAPPA = 5;
+    __device__ static constexpr int gcol(int k, int) { return k; }
+    __device__ static void eval(const ModelPar &P, double t, int N, int k, const double *x, const double *u,
+                                const double *p, double *s, double *C, double *D, double *G)
+    {
+        eval_kappa(P, P.v[KAPPA], t, N, k, x, u, p, s, C, D, G);
+    }
+    __device__ static void eval_kappa(const ModelPar &P, double kap, double, int, int, const double *, const double *u,
+                                      const double *, double *s, double *C, double *D, double *G)
+    {
+        const double adb = P.v[3], amx = P.v[4];
+        const double span = __dsub_rn(amx, adb);
+        const SmoothOr<1> smooth_or(kap, span, {span});
+        for (int i = 0; i < NS * NX; i++) C[i] = 0.0;
+        for (int i = 0; i < NS * NU; i++) D[i] = 0.0;
+        for (int i = 0; i < NS * NG; i++) G[i] = 0.0;
+        const double aa = u[0], ar = u[1];
+        double OR, dOR;
+        smooth_or({__dsub_rn(ar, adb), __dsub_rn(-adb, ar)}, {1.0, -1.0}, OR, dOR);
+        const double ORar = __dmul_rn(OR, ar);
+        const double dORar = __dadd_rn(__dmul_rn(dOR, ar), OR);
+        s[0] = __dsub_rn(aa, ORar);
+        s[1] = __dsub_rn(ORar, aa);
+        D[0 * NU + 0] = 1.0;
+        D[0 * NU + 1] = -dORar;
+        D[1 * NU + 0] = -1.0;
+        D[1 * NU + 1] = dORar;
     }
 };

@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(128, MB) k_discretize_foh(const DiscArgs a)
     // ---- inputs ----
     const double t1 = a.t_grid[k], t2 = a.t_grid[k + 1];
     const double dts = __dsub_rn(t2, t1);
-    double uk[NU], ukp1[NU], pp[NPD];
+    double uk[NU], ukp1[NU], pp[at_least_1(NPD)];
     double xv[NX], xb[NX], xs[NX];
 #pragma unroll
     for (int i = 0; i < NX; i++) xv[i] = a.xd[b * a.xsB + k * a.xsK + i * a.xsE];
@@ -157,7 +157,7 @@ __global__ void __launch_bounds__(128, MB) k_discretize_foh(const DiscArgs a)
 #pragma unroll
             for (int i = 0; i < NU; i++) u[i] = IMP ? 0.0 : cc * uk[i] + omc * ukp1[i];
 
-            double f[NX], A[NX * NX], Bu[NX * NU], Fc[NF * NX];
+            double f[NX], A[NX * NX], Bu[NX * NU], Fc[at_least_1(NF) * NX];
             M::eval(a.par, t, xs, u, pp, f, A, Bu, Fc);
 
             // r = f - A x - B u - F p

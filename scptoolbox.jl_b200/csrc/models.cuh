@@ -8,6 +8,8 @@
 // freeflyer :273-281); packs therefore expose only those NF columns and the parameter
 // index each one belongs to (fcol).  Structural zeros are written as literals so that the
 // fully unrolled consumers constant-fold them away.
+// A model with a fixed final time has no time-dilation column: NF = 0, F = 0 (oscillator), and a pack may read no
+// parameter at all (NPD = 0).  Consumers size their F and p buffers with at_least_1() and never read them then.
 #pragma once
 #include <cuda_runtime.h>
 #include "../../include/scpb.h"
@@ -15,6 +17,9 @@
 struct ModelPar {
     double v[SCPB_MAX_PAR];
 };
+
+// length of a per-model buffer of n elements: C++ has no zero-length arrays, so an empty one keeps one unread element
+__host__ __device__ constexpr int at_least_1(int n) { return n > 0 ? n : 1; }
 
 template <int ID>
 struct Model;
@@ -358,6 +363,32 @@ struct Model<SCPB_MODEL_RENDEZVOUS2D> {
     __device__ __forceinline__ static void post_step(double *) {}
 };
 
+// ---------------------------------------------------------------- forced harmonic oscillator with an input deadband
+// oscillator/definition.jl:161-236, parameters.jl:69-115.  x = [r v]; u[0] = aa, the applied acceleration (the reference
+// acceleration ar and the two one-norm slacks do not enter the dynamics); p = [l1r_1 .. l1r_N] is not read.
+//   f = tf [v; aa - w0^2 r - 2 zeta w0 v]
+// over the FIXED horizon tf: F = 0, so the pack has no active F column (NF = 0) and reads no parameter (NPD = 0).
+// par: zeta, omega0, tf.  The reference's impulse branch (k < 0) is not mirrored: its test runs FOH.
+template <>
+struct Model<SCPB_MODEL_OSCILLATOR> {
+    static constexpr int NX = 2, NU = 4, NF = 0, NPD = 0;
+    static constexpr bool IMPULSE = false;
+    __device__ static constexpr int fcol(int) { return 0; }
+    __device__ __forceinline__ static void eval(const ModelPar &P, double, const double *x, const double *u,
+                                                const double *, double *f, double *A, double *B, double *)
+    {
+        const double zeta = P.v[0], w0 = P.v[1], tf = P.v[2];
+        const double k = -(w0 * w0), c = 2.0 * zeta * w0;
+        f[0] = x[1] * tf;
+        f[1] = (u[0] + (k * x[0] - c * x[1])) * tf;
+        A[0] = 0.0; A[1] = k * tf; A[2] = tf; A[3] = -c * tf;
+#pragma unroll
+        for (int i = 0; i < 8; i++) B[i] = 0.0;
+        B[1] = tf;
+    }
+    __device__ __forceinline__ static void post_step(double *) {}
+};
+
 // ---------------------------------------------------------------- host dispatch on the model id
 template <class M>
 struct ModelId;
@@ -376,6 +407,7 @@ bool with_model(int id, F &&f)
     case SCPB_MODEL_QUADROTOR: f(Model<SCPB_MODEL_QUADROTOR>()); return true;
     case SCPB_MODEL_FREEFLYER: f(Model<SCPB_MODEL_FREEFLYER>()); return true;
     case SCPB_MODEL_RENDEZVOUS2D: f(Model<SCPB_MODEL_RENDEZVOUS2D>()); return true;
+    case SCPB_MODEL_OSCILLATOR: f(Model<SCPB_MODEL_OSCILLATOR>()); return true;
     default: return false;
     }
 }

@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(32) k_propagate_foh(const PropArgs a)
     if (b >= a.B) return;
     const double *ud = a.ud + (size_t)b * a.N * NU;
     double *xc = a.xc + (size_t)b * a.res * NX;
-    double X[NX], pp[NPD];
+    double X[NX], pp[at_least_1(NPD)];
 #pragma unroll
     for (int i = 0; i < NX; i++) { X[i] = a.xd[(size_t)b * a.N * NX + i]; xc[i] = X[i]; }
 #pragma unroll
@@ -59,7 +59,7 @@ __global__ void __launch_bounds__(32) k_propagate_foh(const PropArgs a)
             u[i] = __dadd_rn(__dmul_rn(c, ud[(size_t)(k - 1) * NU + i]), __dmul_rn(omc, ud[(size_t)k * NU + i]));
     };
     auto rhs = [&](double t, const double *x, const double *u, double *f) {
-        double A[NX * NX], Bu[NX * NU], Fc[NF * NX];   // Jacobians are dead code here and removed by the compiler
+        double A[NX * NX], Bu[NX * NU], Fc[at_least_1(NF) * NX];   // Jacobians are dead code here and removed by the compiler
         M::eval(a.par, t, x, u, pp, f, A, Bu, Fc);
     };
 
@@ -106,7 +106,7 @@ __global__ void __launch_bounds__(64) k_propagate_impulse(const PropArgs a, int 
     const int b = (int)(i / nseg), k = (int)(i % nseg);
     const size_t ncol = 1 + (size_t)nseg * subres;
     double *xc = a.xc + (size_t)b * ncol * NX;
-    double X[NX], uk[NU], u0[NU], pp[NPD], jump[NX], Bj[NX * NU];
+    double X[NX], uk[NU], u0[NU], pp[at_least_1(NPD)], jump[NX], Bj[NX * NU];
 #pragma unroll
     for (int j = 0; j < NX; j++) X[j] = a.xd[((size_t)b * a.N + k) * NX + j];
 #pragma unroll
@@ -133,7 +133,7 @@ __global__ void __launch_bounds__(64) k_propagate_impulse(const PropArgs a, int 
         const double tp = __dadd_rn(__dmul_rn(__dsub_rn(1.0, f1), t1), __dmul_rn(f1, t2));
         const double h = __dsub_rn(tp, t), hh = __ddiv_rn(h, 2.0);
         const double tm = __dadd_rn(t, hh), te = __dadd_rn(t, h);
-        double k1[NX], k2[NX], k3[NX], k4[NX], xt[NX], A[NX * NX], Bu[NX * NU], Fc[NF * NX];
+        double k1[NX], k2[NX], k3[NX], k4[NX], xt[NX], A[NX * NX], Bu[NX * NU], Fc[at_least_1(NF) * NX];
         M::eval(a.par, t, X, u0, pp, k1, A, Bu, Fc);
 #pragma unroll
         for (int j = 0; j < NX; j++) xt[j] = X[j] + hh * k1[j];

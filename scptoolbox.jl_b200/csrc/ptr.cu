@@ -635,7 +635,7 @@ __global__ void k_gusto_nodes(const GustoDev d)
     const double *xr = d.xd + ((size_t)b * d.N + k) * NX, *ur = d.ud + ((size_t)b * d.N + k) * NU, *pr = d.p + (size_t)b * d.np;
     const double *xs = d.xn + ((size_t)b * d.N + k) * NX, *us = d.un + ((size_t)b * d.N + k) * NU, *ps = d.pn + (size_t)b * d.np;
     const double t = d.t_grid[k];
-    double f[NX], A[NX * NX], Bm[NX * NU], F[NX * NF], fl[NX];
+    double f[NX], A[NX * NX], Bm[NX * NU], F[NX * at_least_1(NF)], fl[NX];
     M::eval(d.par, t, xr, ur, pr, f, A, Bm, F);
     for (int r = 0; r < NX; r++) {           // f_lin(sol) = f(ref) + A (xs - xr) + B (us - ur) + F (ps - pr)
         double a = f[r];
@@ -800,7 +800,8 @@ static int debug_constr_t(scpb_handle_s *h, int B, int N, int ns, int ng, const 
     return rc;
 }
 
-// GuSTO's node terms with the problem's model and pack; SCPB_ERR_UNSUPPORTED for the rendezvous, which GuSTO lacks
+// GuSTO's node terms with the problem's model and pack; SCPB_ERR_UNSUPPORTED for the rendezvous and the oscillator,
+// whose deadband packs GuSTO lacks
 static int launch_gusto_nodes(scpb_ptr_s *s, const GustoDev &gd, cudaStream_t st)
 {
     const int nbn = (int)(((long long)gd.B * gd.N + 63) / 64);
@@ -808,7 +809,7 @@ static int launch_gusto_nodes(scpb_ptr_s *s, const GustoDev &gd, cudaStream_t st
     with_model(s->model_id, [&](auto m) {
         using M = decltype(m);
         constexpr int id = ModelId<M>::value;
-        if constexpr (id != SCPB_MODEL_RENDEZVOUS2D) {
+        if constexpr (id != SCPB_MODEL_RENDEZVOUS2D && id != SCPB_MODEL_OSCILLATOR) {
             if (s->d.ns > 0) k_gusto_nodes<M, PackOf<id>><<<nbn, 64, 0, st>>>(gd);
             else k_gusto_nodes<M, Constr<0>><<<nbn, 64, 0, st>>>(gd);
             rc = SCPB_OK;
@@ -1050,7 +1051,14 @@ int32_t scpb_ptr_setup(scpb_handle h, scpb_cone cone, const scpb_ptr_desc *desc,
                            desc->ns, desc->ng);
         if (h->model_id == SCPB_MODEL_FREEFLYER && desc->np != 1 + Constr<SCPB_MODEL_FREEFLYER>::NISS * desc->N)
             return set_err(h, SCPB_ERR_ARG, "ptr_setup: the free-flyer pack expects np = 1 + 6 N");
+        if (h->model_id == SCPB_MODEL_OSCILLATOR && desc->np != desc->N)
+            return set_err(h, SCPB_ERR_ARG, "ptr_setup: the oscillator pack expects np = N (one parameter per node)");
     }
+    int nf = -1;   // the DLTV's F block holds the pack's active columns only
+    with_model(h->model_id, [&](auto m) { nf = decltype(m)::NF; });
+    if (desc->nf != nf)
+        return set_err(h, SCPB_ERR_ARG, "ptr_setup: model %d has %d active F columns, the descriptor %d", h->model_id, nf,
+                       desc->nf);
     if (desc->method != SCPB_FOH && desc->method != SCPB_IMPULSE)
         return set_err(h, SCPB_ERR_ARG, "ptr_setup: unknown discretization method %d", desc->method);
     // refused here rather than at the first discretize! of a solve: only the rendezvous pack has impulse semantics

@@ -86,7 +86,7 @@ static void julia_views(DiscArgs &a, int nx, int nu, int np, double *A, double *
 
 extern "C" {
 
-int32_t scpb_version(void) { return 102; }
+int32_t scpb_version(void) { return 103; }
 
 int32_t scpb_create(int32_t device, scpb_handle *out)
 {
@@ -210,7 +210,8 @@ int32_t scpb_discretize(scpb_handle h, int32_t method, int32_t B, int32_t N, int
     SCPB_CUDA(h, cudaMemcpyAsync(d_u, ud, sizeof(double) * s_u, cudaMemcpyHostToDevice, st));
     SCPB_CUDA(h, cudaMemcpyAsync(d_p, p, sizeof(double) * s_p, cudaMemcpyHostToDevice, st));
     SCPB_CUDA(h, cudaMemcpyAsync(d_s, iSx_diag, sizeof(double) * s_s, cudaMemcpyHostToDevice, st));
-    // inactive columns of the dense F stay zero (F has np columns, only the time-dilation ones are written)
+    // inactive columns of the dense F stay zero (F has np columns, only the time-dilation ones are written; a model with
+    // a fixed final time has none, and F stays all zeros)
     SCPB_CUDA(h, cudaMemsetAsync(d_F, 0, sizeof(double) * s_F, st));
     DiscArgs a{};
     a.B = B; a.N = N; a.Nsub = Nsub;

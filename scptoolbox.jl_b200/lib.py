@@ -15,6 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.environ.get("SCPB_LIBRARY") or os.path.join(HERE, "libscpb.so")   # override: A/B runs of kernel variants
 
 MODEL_DBLINT, MODEL_ROCKET, MODEL_STARSHIP, MODEL_QUADROTOR, MODEL_FREEFLYER, MODEL_RENDEZVOUS2D = 1, 2, 3, 4, 5, 6
+MODEL_OSCILLATOR = 7
 FOH, IMPULSE = 0, 1
 
 _lib = None
