@@ -110,7 +110,6 @@ struct Ctx {
                                             // the substitution vector: int offsets into the dynamic shared window
     int Rmax;
     int *flag;                          // shared scratch word for CTA-uniform decisions
-    long long t_fw, t_bw, t_ldl_n;      // cycle counters (CTA-local copies, meaningful on thread 0)
     long long *lprof;                   // thread 0 of CTA 0: per-level cycles [factor | forward | backward][nlevels]
     int sn;                             // supernodal mode
     double *Ypanels;                    // supernodal mode: this group's panels (the Y array, one seed after the other)
@@ -168,6 +167,13 @@ __device__ __forceinline__ void seed_reduce(const Ctx &c, double (&v)[K], int op
 }
 
 #define GI(e) ((size_t)(e) * G + sg)
+
+// cycle counters of the solve (written to IpmData.prof by thread 0 of CTA 0).  Only thread 0 keeps them, in shared
+// memory: as per-thread registers they were live across every call of the level programs and took registers from them.
+//   [0..7] phases (k_ipm_solve, PROF), [8] forward substitutions, [9] backward ones, [10] substitutions,
+//   [11] factorisations, [12] repeated factorisations, [13] last phase stamp, [14] start, [15] substitution stamp
+__shared__ long long ipm_s_prof[16];
+#define IPM_STAMP(k) { if (threadIdx.x == 0) ipm_s_prof[k] = clock64(); }
 
 __device__ __forceinline__ void set_lanes(Ctx &c, int R)
 {
@@ -267,7 +273,7 @@ __device__ __forceinline__ void kkt_assemble(const IpmProgram &P, const Ctx &c, 
 // backward sweep, row order for the forward sweep).  Combine-only items (flag 4, the hybrid program's bridge level) just
 // write their combined target back.  No fence, no atomic: the level's barrier orders the slots.
 // The program data of the next phase (item descriptors, op indices) is requested one phase early.
-// Separate (noinline) function with by-value arguments: see solve_sweep.
+// Separate (noinline) function with its arguments in shared memory: see ipm_fa.
 #define IPM_FPF CONIC_FACTOR_PF
 // Substitutions: an item of a split target stores its partial sum in its slot and counts itself in; the last item of
 // the target to finish subtracts all slots from the target in slot order (and resets the counter), so the sum does not
@@ -288,30 +294,40 @@ __device__ __forceinline__ double ipm_split_sum(const double *part, int k0, int 
     for (int k = k0; k < k1; k++) acc -= part[k * G + sg];
     return acc;
 }
-struct FactorArgs {
+struct FactorArgs {   // CTA-uniform: one block per launch in shared memory (ipm_fa)
     const int4 *fa_item, *fb_item;
     const int2 *ft_op;
     const int4 *fb_cmb;             // per phase-B item: slot ranges of its entry and of its pivot
     double *Y, *Ls, *Lrow, *invD;   // group-blocked, already offset to this CTA's group
     double *part;                   // partial sums of the level's split targets (shared or global memory)
     int o_fal, o_faR, o_fbl;        // offsets (ints) into the dynamic shared memory window
-    int nl, nnzLd, G, sg, slot, nslots;
-    long long *lprof;
+    int nl, nnzLd, G, nslots;
+    long long *lprof;               // per-level cycle counters of CTA 0 (written by its thread 0) or nullptr
 };
 extern __shared__ int ipm_smem[];
 // per-seed regularisation state of the factorisation, file-scope shared so that the noinline level programs reach it
-// without widening their by-value argument blocks (a block above 128 bytes is passed through local memory)
 __shared__ double ipm_s_delta[IPM_MAXG];   // static regularisation of each seed of the group
 __shared__ int ipm_s_bad[IPM_MAXG];        // "inertia lost" flags raised by the factorisation
 __shared__ double ipm_s_reg[2];            // rho_min, bad_abs
+// The factorisation's arguments live in shared memory (filled once per launch), not in registers.  A subroutine called
+// inside the solver's loops gets less than the 64 registers of a 1024-thread CTA (the body keeps some of its values in
+// registers across the call); a by-value block plus the phase-A pipeline did not fit, and what does not fit is spilled
+// to local memory inside the pass loops.  Loads from the block after a barrier are reissued (the barrier orders shared
+// memory), so the phase-B pointers and the profile state take no register across phase A.  The group size G is a
+// compile-time constant (one inlined copy per G behind the one call site, kkt_factor_levels) and all indices are 32-bit
+// element offsets into this group's arrays, so the index arithmetic needs no 64-bit or multiply temporaries.
+__shared__ FactorArgs ipm_fa;
+__shared__ long long ipm_lvl_t;            // thread 0 of CTA 0: cycle counter at the end of the previous level
 
-__device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
+template <int G>
+__device__ __forceinline__ void kkt_factor_levels_g()
 {
+    const FactorArgs &a = ipm_fa;
     __builtin_assume(__isGlobal(a.fa_item)); __builtin_assume(__isGlobal(a.fb_item)); __builtin_assume(__isGlobal(a.ft_op));
     __builtin_assume(__isGlobal(a.Y)); __builtin_assume(__isGlobal(a.Ls)); __builtin_assume(__isGlobal(a.Lrow));
     __builtin_assume(__isGlobal(a.invD));
+    const int sg = threadIdx.x & (G - 1), slot = threadIdx.x / G, nslots = a.nslots;
     const int *fal = ipm_smem + a.o_fal, *faR = ipm_smem + a.o_faR, *fbl = ipm_smem + a.o_fbl;
-    const int G = a.G, sg = a.sg, slot = a.slot, nslots = a.nslots;
     // three-stage software pipeline over the passes of phase A: the item descriptor of pass p+2 and the op indices of
     // pass p+1 are requested while the gathers of pass p are in flight, so a pass costs one memory latency
     int t_tgt;                 // current pass: target, or partial-sum slot | 1 << 30 for a split target, or -1
@@ -339,21 +355,18 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
     IPM_FA_ITEM(0, 0)
     IPM_FA_OPS(t_tgt, t_op, faR[0])
     IPM_FA_ITEM(0, (nslots >> (31 - __clz(faR[0]))))
-    long long tl_ = a.lprof ? clock64() : 0;
+    if (threadIdx.x == 0 && a.lprof) ipm_lvl_t = clock64();
     for (int lv = 0; lv < a.nl; lv++) {
         // ---- phase A ----
         const int R = faR[lv], nisl = nslots >> (31 - __clz(R));
         const int nA = fal[lv + 1] - fal[lv];
-        const int b0 = fbl[lv], b1 = fbl[lv + 1];
-        int4 sc = make_int4(-1, 0, 0, 0), sr = make_int4(0, 0, 0, 0);   // first phase-B item of this lane and its slot
-        if (b0 + slot < b1) { sc = a.fb_item[b0 + slot]; sr = a.fb_cmb[b0 + slot]; }   // ranges, requested early
         for (int off = 0; off < nA; off += nisl) {
             double ya_[IPM_FPF], la_[IPM_FPF];
 #pragma unroll
             for (int j = 0; j < IPM_FPF; j++) {
                 const bool on_ = t_op[j].x >= 0;
-                ya_[j] = on_ ? __ldcg(&a.Y[(size_t)t_op[j].x * G + sg]) : 0.0;
-                la_[j] = on_ ? a.Lrow[(size_t)t_op[j].y * G + sg] : 0.0;   // row order: consecutive within an item
+                ya_[j] = on_ ? __ldcg(&a.Y[t_op[j].x * G + sg]) : 0.0;
+                la_[j] = on_ ? a.Lrow[t_op[j].y * G + sg] : 0.0;   // row order: consecutive within an item
             }
             int n_tgt; int2 n_op[IPM_FPF];
             IPM_FA_OPS(n_tgt, n_op, R)                       // pass p+1 (descriptor requested one pass ago)
@@ -364,29 +377,33 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
             for (int o_ = G; o_ < G * R; o_ <<= 1) part_ += __shfl_xor_sync(0xffffffffu, part_, o_);
             if (t_tgt >= 0 && (slot & (R - 1)) == 0) {
                 if (t_tgt >> 30) a.part[(t_tgt & 0x3fffffff) * G + sg] = part_;   // phase B combines it
-                else { double *p_ = &a.Y[(size_t)t_tgt * G + sg]; *p_ = __ldcg(p_) - part_; }
+                else { double *p_ = &a.Y[t_tgt * G + sg]; *p_ = __ldcg(p_) - part_; }
             }
             t_tgt = n_tgt;
 #pragma unroll
             for (int j = 0; j < IPM_FPF; j++) t_op[j] = n_op[j];
         }
-        // descriptor of the next level's first pass: in flight across the barrier and phase B
+        // first phase-B item of this lane and its slot ranges, and the descriptor of the next level's first pass: in
+        // flight across the barrier
+        const int b0 = fbl[lv], b1 = fbl[lv + 1];
+        int4 sc = make_int4(-1, 0, 0, 0), sr = make_int4(0, 0, 0, 0);
+        if (b0 + slot < b1) { sc = a.fb_item[b0 + slot]; sr = a.fb_cmb[b0 + slot]; }
         if (lv + 1 < a.nl) IPM_FA_ITEM(lv + 1, 0)
         __syncthreads();
         // ---- phase B: one latency per pass (the next item is requested while the current loads are in flight) ----
         for (int w = b0 + slot; w < b1; w += nslots) {
             const double sgn = (sc.w & 1) ? 1.0 : -1.0;
             const bool isd = (sc.w & 2) != 0;
-            double e = __ldcg(&a.Y[(size_t)sc.x * G + sg]);
-            double d = isd ? 0.0 : __ldcg(&a.Y[(size_t)(a.nnzLd + sc.y) * G + sg]);
+            double e = __ldcg(&a.Y[sc.x * G + sg]);
+            double d = isd ? 0.0 : __ldcg(&a.Y[(a.nnzLd + sc.y) * G + sg]);
             const int4 cur = sc, cr = sr;
             if (w + nslots < b1) { sc = a.fb_item[w + nslots]; sr = a.fb_cmb[w + nslots]; }
             e = ipm_split_sum(a.part, cr.x, cr.y, e, G, sg);
             if (isd) d = e;
             else {
                 d = ipm_split_sum(a.part, cr.z, cr.w, d, G, sg);
-                if (cr.y > cr.x) a.Y[(size_t)cur.x * G + sg] = e;   // a later level reads it as an operand
-                if (cur.w & 4) continue;                            // combine-only item
+                if (cr.y > cr.x) a.Y[cur.x * G + sg] = e;   // a later level reads it as an operand
+                if (cur.w & 4) continue;                // combine-only item
             }
             const double dl_ = ipm_s_delta[sg];
             if (!(sgn * d > 0.5 * dl_)) {   // dynamic regularisation keeps the expected inertia
@@ -394,11 +411,11 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
                 d = sgn * fmax(dl_, ipm_s_reg[0]);
             }
             const double inv = 1.0 / d;
-            if (isd) a.invD[(size_t)cur.y * G + sg] = inv;
+            if (isd) a.invD[cur.y * G + sg] = inv;
             else {
                 const double lv_ = e * inv;
-                a.Ls[(size_t)cur.x * G + sg] = lv_;
-                a.Lrow[(size_t)cur.z * G + sg] = lv_;
+                a.Ls[cur.x * G + sg] = lv_;
+                a.Lrow[cur.z * G + sg] = lv_;
             }
         }
         if (lv + 1 < a.nl) {   // op indices of the next level's first pass, descriptor of its second pass
@@ -407,17 +424,26 @@ __device__ __noinline__ void kkt_factor_levels(const FactorArgs a)
             IPM_FA_ITEM(lv + 1, (nslots >> (31 - __clz(Rn))))
         }
         __syncthreads();
-        if (a.lprof) { const long long tn = clock64(); a.lprof[lv] += tn - tl_; tl_ = tn; }
+        if (threadIdx.x == 0 && a.lprof) { const long long tn = clock64(); a.lprof[lv] += tn - ipm_lvl_t; ipm_lvl_t = tn; }
     }
 #undef IPM_FA_ITEM
 #undef IPM_FA_OPS
+}
+__device__ __noinline__ void kkt_factor_levels()
+{
+    switch (ipm_fa.G) {
+        case 1: kkt_factor_levels_g<1>(); break;
+        case 2: kkt_factor_levels_g<2>(); break;
+        case 4: kkt_factor_levels_g<4>(); break;
+        default: kkt_factor_levels_g<8>(); break;
+    }
 }
 
 // supernodal numeric factorisation: one thread (small leaves) or one lane group (8, 16 or 32 lanes, by panel height)
 // per (supernode, seed) item, one barrier per supernodal level; panels live in registers (conic_sn.cuh).  The
 // descriptor of a unit's next item is requested before the current item is worked on.
-// Like the scalar programs these are separate (noinline) functions with BY-VALUE arguments: passing the solver's
-// context or the kernel parameters by reference would force them into local memory for the whole kernel.
+// Like the scalar programs these are separate (noinline) functions whose arguments come from shared memory: passing the
+// solver's context or the kernel parameters by reference would force them into local memory for the whole kernel.
 struct SnArgs {
     SnProgram sn;
     double *Y, *invD, *vs;          // this group's panels (one seed after the other), 1/D (group-blocked), shared vector
@@ -508,18 +534,17 @@ __device__ __forceinline__ void kkt_ldl_solve_sn(const IpmProgram &P, Ctx &c, co
 {
     const int G = c.G, sg = c.sg;
     double *vs = c.vs;
-    const long long t0_ = clock64();
+    IPM_STAMP(15)
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
     __syncthreads();
     kkt_sweep_sn<1>(c.s_sn, c.tid);
-    const long long t1_ = clock64();
+    if (c.tid == 0) { const long long t1_ = clock64(); ipm_s_prof[8] += t1_ - ipm_s_prof[15]; ipm_s_prof[15] = t1_; }
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] *= invD[GI(i)];
     __syncthreads();
     kkt_sweep_sn<-1>(c.s_sn, c.tid);
     for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] = vs[i * G + sg];
     __syncthreads();
-    const long long t2_ = clock64();
-    c.t_fw += t1_ - t0_; c.t_bw += t2_ - t1_; c.t_ldl_n += 1;
+    if (c.tid == 0) { ipm_s_prof[9] += clock64() - ipm_s_prof[15]; ipm_s_prof[10] += 1; }
 }
 
 // ---- hybrid program: the top supernodes (conic_sn.cuh, hy_*), one warp per (supernode, seed) item, one barrier per
@@ -555,7 +580,7 @@ __device__ __forceinline__ void hy_for_items(const HyArgs &a, int tl, int tid, F
 
 __device__ __noinline__ void kkt_factor_top(const HyArgs *ap, int tid)
 {
-    const HyArgs a = *ap;
+    const HyArgs &a = *ap;   // read in place: a register copy of the whole block is spilled at 1024 threads
     long long *lp = (tid == 0) ? a.lprof : nullptr;
     long long tl_ = lp ? clock64() : 0;
     for (int tl = 0; tl < a.hy.ntl; tl++) {
@@ -571,7 +596,7 @@ __device__ __noinline__ void kkt_factor_top(const HyArgs *ap, int tid)
 template <int DIR>
 __device__ __noinline__ void kkt_sweep_top(const HyArgs *ap, int tid)
 {
-    const HyArgs a = *ap;
+    const HyArgs &a = *ap;
     double *vs = (double *)(ipm_smem + a.o_vs);
     long long *lp = (tid == 0 && a.lprof) ? a.lprof + (DIR > 0 ? 1 : 2) * a.hy.ntl : nullptr;
     long long tl_ = lp ? clock64() : 0;
@@ -587,16 +612,10 @@ __device__ __noinline__ void kkt_sweep_top(const HyArgs *ap, int tid)
 // SN (compile time): the supernodal kernels are instantiated only in the kernel variant that uses them -- their mere
 // presence as call sites costs the default (scalar) variant ~3 KB of spill traffic per thread (ptxas -v)
 template <int SN>
-__device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *Y, double *Ls, double *invD)
+__device__ __forceinline__ void kkt_factor(const Ctx &c)
 {
     if constexpr (SN == 1) { kkt_factor_sn(c.s_sn, c.tid); return; }
-    FactorArgs a;
-    a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fb_cmb = P.fb_cmb;
-    a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.fpart;
-    a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
-    a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = c.G; a.sg = c.sg; a.slot = c.slot; a.nslots = c.nslots;
-    a.lprof = c.lprof;
-    kkt_factor_levels(a);
+    kkt_factor_levels();
     if constexpr (SN == 2) kkt_factor_top(c.s_hy, c.tid);
 }
 
@@ -608,8 +627,8 @@ __device__ __forceinline__ void kkt_factor(const IpmProgram &P, Ctx &c, double *
 // Items of a split row store their partial sums in slots that the last of them subtracts in slot order
 // (ipm_split_done); the slots and counters of a level live in shared memory after the vector (global memory when they
 // do not fit).
-// The sweep is a separate (noinline) function with by-value arguments and shared-window pointers: its register
-// allocation is independent of the 60+ live pointers of the solver body, so the prefetch registers are not spilled
+// The sweep is a separate (noinline) function whose arguments live in shared memory (ipm_sw, like ipm_fa): its
+// register allocation is separate from the solver body's, and no argument block occupies registers across the levels
 // (a spilled prefetch is a synchronous load).
 #define IPM_PF CONIC_SOLVE_PF
 struct SweepArgs {
@@ -620,17 +639,20 @@ struct SweepArgs {
     double *part;           // partial sums of the level's split rows / columns, and their counters
     unsigned *pcnt;
     int o_lvl, o_R, o_vs;   // offsets (ints) into the dynamic shared memory window
-    int nl, lv0, G, sg, slot, nslots;
-    long long *lprof;       // per-level cycle counters (CTA 0, thread 0) or nullptr
+    int nl, lv0, G, nslots;
+    long long *lprof;       // per-level cycle counters of CTA 0 (written by its thread 0) or nullptr
 };
+// forward and backward sweep arguments, CTA-uniform, filled once per launch (see ipm_fa)
+__shared__ SweepArgs ipm_sw[2];
 
 template <int DIR>
-__device__ __noinline__ void solve_sweep(const SweepArgs a)
+__device__ __noinline__ void solve_sweep()
 {
+    const SweepArgs &a = ipm_sw[DIR > 0 ? 0 : 1];
     __builtin_assume(__isGlobal(a.items)); __builtin_assume(__isGlobal(a.idxarr)); __builtin_assume(__isGlobal(a.vals));
     const int *lvl = ipm_smem + a.o_lvl, *Rl = ipm_smem + a.o_R;
     double *vs = (double *)(ipm_smem + a.o_vs);
-    const int G = a.G, sg = a.sg, slot = a.slot;
+    const int G = a.G, sg = threadIdx.x & (G - 1), slot = threadIdx.x >> (31 - __clz(G));
     const int nsteps = DIR > 0 ? a.nl - a.lv0 : a.lv0 + 1;
     if (nsteps <= 0) return;
     // item descriptor of this lane for the level after next; node (or partial-sum slot | 1 << 30), first entry, end
@@ -676,7 +698,7 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
     IPM_VALS_LOAD()
     if (nsteps > 1) IPM_ITEM_LOAD(a.lv0 + DIR, 0) else i_node = -1;
     __syncthreads();
-    long long tl_ = a.lprof ? clock64() : 0;
+    if (threadIdx.x == 0 && a.lprof) ipm_lvl_t = clock64();
     for (int st = 0, lv = a.lv0; st < nsteps; st++, lv += DIR) {
         const int R = Rl[lv], nisl = a.nslots >> (31 - __clz(R));
         IPM_CONSUME(R)
@@ -694,7 +716,7 @@ __device__ __noinline__ void solve_sweep(const SweepArgs a)
         IPM_VALS_LOAD()
         if (st + 2 < nsteps) IPM_ITEM_LOAD(lv + 2 * DIR, 0) else i_node = -1;
         __syncthreads();
-        if (a.lprof) { const long long tn = clock64(); a.lprof[lv] += tn - tl_; tl_ = tn; }
+        if (threadIdx.x == 0 && a.lprof) { const long long tn = clock64(); a.lprof[lv] += tn - ipm_lvl_t; ipm_lvl_t = tn; }
     }
 #undef IPM_ITEM_LOAD
 #undef IPM_VALS_LOAD
@@ -706,30 +728,21 @@ __device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c, 
 {
     const int G = c.G, sg = c.sg;
     double *vs = c.vs;
-    const long long t0_ = clock64();
+    IPM_STAMP(15)
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
-    SweepArgs a;
-    a.nl = P.nlevels; a.G = G; a.sg = sg; a.slot = c.slot; a.nslots = c.nslots; a.o_vs = c.o_vs; a.part = c.spart; a.pcnt = c.pcnt;
-    // forward: level 0 rows are empty (leaves have no dependencies); the barrier inside the sweep publishes vs
-    a.items = P.fwp_item; a.idxarr = P.Lr_col; a.vals = c.Lrow; a.o_lvl = c.o_fwl; a.o_R = c.o_fwR; a.lv0 = 1;
-    a.cmb = P.fwc_item;
-    a.lprof = c.lprof ? c.lprof + P.nlevels : nullptr;
-    solve_sweep<1>(a);
+    // forward (level 0 rows are empty: leaves have no dependencies); the barrier inside the sweep publishes vs
+    solve_sweep<1>();
     if (P.nlevels <= 1) __syncthreads();
     if constexpr (SN == 2) kkt_sweep_top<1>(c.s_hy, c.tid);   // after the bridge level: column-oriented top panels
-    const long long t1_ = clock64();
+    if (c.tid == 0) { const long long t1_ = clock64(); ipm_s_prof[8] += t1_ - ipm_s_prof[15]; ipm_s_prof[15] = t1_; }
     for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] *= invD[GI(i)];
     if constexpr (SN == 2) { __syncthreads(); kkt_sweep_top<-1>(c.s_hy, c.tid); }
-    // backward: the top level holds roots only (empty columns)
-    a.items = P.bwp_item; a.idxarr = P.L_ri; a.vals = Ls; a.o_lvl = c.o_bwl; a.o_R = c.o_bwR; a.lv0 = P.nlevels - 2;
-    a.cmb = P.bwc_item;
-    a.lprof = c.lprof ? c.lprof + 2 * P.nlevels : nullptr;
-    solve_sweep<-1>(a);
+    // backward (the top level holds roots only: empty columns)
+    solve_sweep<-1>();
     if (P.nlevels <= 1) __syncthreads();
     for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] = vs[i * G + sg];
     __syncthreads();
-    const long long t2_ = clock64();
-    c.t_fw += t1_ - t0_; c.t_bw += t2_ - t1_; c.t_ldl_n += 1;
+    if (c.tid == 0) { ipm_s_prof[9] += clock64() - ipm_s_prof[15]; ipm_s_prof[10] += 1; }
 }
 
 // in-place solve of (L D L') v = rhs on the permuted vector v
@@ -1142,7 +1155,6 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
     c.G = D.G; c.tid = threadIdx.x; c.sg = c.tid % c.G; c.slot = c.tid / c.G; c.nslots = NT / c.G; c.nwarps = NT / 32;
     c.flag = &s_flag; c.reftol = O.reftol; c.s_mu = s_mu; c.mu_tight = O.mu_tight;
     c.Rmax = D.R;
-    c.t_fw = c.t_bw = c.t_ldl_n = 0;
     c.lprof = (blockIdx.x == 0 && threadIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 : nullptr;
     if (c.lprof) for (int i = 0; i < 3 * (P.nlevels + (SN == 2 ? P.hy.ntl : 0)); i++) c.lprof[i] = 0;
     set_lanes(c, c.Rmax);
@@ -1197,14 +1209,32 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         c.fpart = c.spart = GP(D.part, P.npart + 1);
         c.pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
     }
+    if (SN != 1 && threadIdx.x == 0) {
+        FactorArgs a;
+        a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fb_cmb = P.fb_cmb;
+        a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.fpart;
+        a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
+        a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = G; a.nslots = c.nslots;
+        a.lprof = c.lprof;   // thread 0 of CTA 0 only (c.lprof is nullptr everywhere else)
+        ipm_fa = a;
+        SweepArgs w;
+        w.nl = P.nlevels; w.G = G; w.nslots = c.nslots; w.o_vs = c.o_vs; w.part = c.spart; w.pcnt = c.pcnt;
+        w.items = P.fwp_item; w.idxarr = P.Lr_col; w.vals = c.Lrow; w.o_lvl = c.o_fwl; w.o_R = c.o_fwR; w.lv0 = 1;
+        w.cmb = P.fwc_item;
+        w.lprof = c.lprof ? c.lprof + P.nlevels : nullptr;
+        ipm_sw[0] = w;
+        w.items = P.bwp_item; w.idxarr = P.L_ri; w.vals = Ls; w.o_lvl = c.o_bwl; w.o_R = c.o_bwR; w.lv0 = P.nlevels - 2;
+        w.cmb = P.bwc_item;
+        w.lprof = c.lprof ? c.lprof + 2 * P.nlevels : nullptr;
+        ipm_sw[1] = w;
+    }
 #undef GP
 
-    long long pt[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    long long n_fact = 0;   // factorisations (= interior-point iterations) of this CTA
-    long long n_retry = 0;  // ... and the repeated ones (static regularisation escalated)
-    long long tq = clock64();
-    const long long tstart = tq;
-#define PROF(i) { const long long tn = clock64(); pt[i] += tn - tq; tq = tn; }
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < 13; i++) ipm_s_prof[i] = 0;
+        ipm_s_prof[13] = ipm_s_prof[14] = clock64();
+    }
+#define PROF(i) { if (threadIdx.x == 0) { const long long tn = clock64(); ipm_s_prof[i] += tn - ipm_s_prof[13]; ipm_s_prof[13] = tn; } }
     if (c.tid < G) {
         const int sd = (int)g * G + c.tid;
         // padded seeds and seeds the caller marked (SCP seeds that have already stopped) are not solved
@@ -1224,7 +1254,7 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
     }
     if (D.debug_kkt) {   // test hook: one KKT solve on the device with the caller's scaling and right-hand side
         kkt_assemble(P, c, D, Av, Gv, wm, Y, 0.0);
-        kkt_factor<SN>(P, c, Y, Ls, invD);
+        kkt_factor<SN>(c);
         kkt_ldl_solve<SN>(P, c, Ls, invD, rhs);
         if (c.tid < G && (int)g * G + c.tid < D.B) D.status[(int)g * G + c.tid] = s_bad[c.tid];
         return;
@@ -1235,7 +1265,7 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
     for (int tr_ = 0;; tr_++) {                                                                    \
         if (c.tid < G) s_bad[c.tid] = 0;                                                           \
         kkt_assemble(P, c, D, Av, Gv, wm, Y, 0.0);                                                 \
-        kkt_factor<SN>(P, c, Y, Ls, invD);                                                             \
+        kkt_factor<SN>(c);                                                                         \
         if (c.tid == 0) {                                                                          \
             int again_ = 0;                                                                        \
             for (int q = 0; q < G; q++)                                                            \
@@ -1248,7 +1278,7 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         const int again_ = s_flag;                                                                 \
         __syncthreads();                                                                           \
         if (!again_ || tr_ >= 4) break;                                                            \
-        n_retry++;                                                                                 \
+        if (c.tid == 0) ipm_s_prof[12]++;                                                          \
     }
     if (O.equil > 0) equilibrate(P, c, Av, Gv, cc, bb, hh, eqD, eqA, eqG, O.equil);
     PROF(0)
@@ -1454,7 +1484,7 @@ restart_cold:
         PROF(3)
         IPM_FACTOR()
         PROF(4)
-        n_fact++;
+        if (c.tid == 0) ipm_s_prof[11]++;
 
         // ---- affine direction: bx=-rx, by=-ry, bz=-rz+s ; ds = -s - W^2 dz ----
         for (int i = c.slot; i < P.n; i += c.nslots) r1[GI(i)] = -rx[GI(i)];
@@ -1545,9 +1575,9 @@ restart_cold:
         PROF(6)
     }
     if (blockIdx.x == 0 && threadIdx.x == 0 && D.prof) {
-        pt[7] = clock64() - tstart;
-        for (int i = 0; i < 8; i++) D.prof[i] = pt[i];
-        D.prof[8] = c.t_fw; D.prof[9] = c.t_bw; D.prof[10] = c.t_ldl_n; D.prof[11] = n_fact | (n_retry << 32);
+        ipm_s_prof[7] = clock64() - ipm_s_prof[14];
+        for (int i = 0; i < 11; i++) D.prof[i] = ipm_s_prof[i];
+        D.prof[11] = ipm_s_prof[11] | (ipm_s_prof[12] << 32);
     }
 #undef PROF
     // ---- a warm-started seed that did not reach the tolerances: the group starts again from the cold starting point ----
