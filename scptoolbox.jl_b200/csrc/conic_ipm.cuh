@@ -112,24 +112,37 @@ struct Ctx {
     int *flag;                          // shared scratch word for CTA-uniform decisions
     long long *lprof;                   // thread 0 of CTA 0: per-level cycles [factor | forward | backward][nlevels]
     int sn;                             // supernodal mode
-    double *Ypanels;                    // supernodal mode: this group's panels (the Y array, one seed after the other)
     const struct SnArgs *s_sn;          // supernodal mode: argument block of the panel kernels, in shared memory
     const struct HyArgs *s_hy;          // hybrid mode: argument block of the top-panel phases, in shared memory
     size_t ysize;                       // doubles per seed of the Y array
     const int *s_done;                  // shared: per-seed "finished" flags (finished seeds skip the per-seed panel work)
     double *s_delta;                    // shared: per-seed static regularisation
     int *s_bad;                         // shared: per-seed "inertia lost" flag raised by the factorisation
-    double rho_min, bad_abs;
-    double *vs;                         // shared-memory substitution vector (nullptr: use global memory)
-    double *Lrow;                       // row-ordered copy of the scaled factor (forward substitution)
-    double *fpart, *spart;              // partial sums of the split targets of a level: factorisation, substitutions
-    unsigned *pcnt;                     // ... and the substitutions' finished-item counters
-    double reftol;                      // iterative refinement stops once |residual|_inf <= reftol*(1+|rhs|_inf) ...
-    const double *s_mu;                 // ... reftol while the seed's complementarity gap/deg is above mu_tight, 1e-13 below it
-    double mu_tight;                    //     (shared: per-seed mu of the current iterate)
+    const double *s_mu;                 // shared: per-seed mu (complementarity gap / deg) of the current iterate
     double *red;   // shared: [10][IPM_NT_MAX/32][IPM_MAXG]
     double *out;   // shared: [10][IPM_MAXG]
 };
+
+// This CTA's group arrays (group-blocked, already offset to the group) and the CTA-uniform scalars of the solve, in
+// shared memory, filled by thread 0 once per launch.  As 64-bit bases in every thread's registers they do not fit the 64
+// registers of a 1024-thread CTA: they end up in a per-thread stack frame (312 KB of local memory per CTA) that the
+// loops reload mostly from L2, and what the body keeps live across the level programs' calls is taken from their
+// registers.  A base read from here where it is used costs one shared load, and a barrier ends its life (the barrier
+// orders shared memory, so the load is issued again after it).
+struct IpmGroup {
+    double *Av, *Gv, *cc, *bb, *hh;   // equilibrated problem data
+    double *x, *y, *z, *s, *eqD, *eqA, *eqG, *xb, *yb, *zb, *sb;
+    double *rx, *ry, *rz, *lam, *wm, *socw, *soceta;
+    double *dx, *dy, *dz, *ds, *dsa, *dza, *tm, *gm, *r1, *r2, *e1, *rhs, *Y, *Ls, *invD;
+    double *vs;                       // shared-memory substitution vector (nullptr: the sweeps work in global memory)
+    double reftol;                    // iterative refinement stops once |residual|_inf <= reftol*(1+|rhs|_inf) while the
+    double mu_tight;                  // seed's mu is above mu_tight, and at min(reftol, 1e-13) below it
+};
+__shared__ IpmGroup ipm_ar;
+// A base read from shared memory is a generic pointer to the compiler: without this it would issue generic loads and
+// stores, and take every store through such a pointer as one that may change the shared blocks
+template <class T>
+__device__ __forceinline__ T *glb(T *p) { __builtin_assume(__isGlobal(p)); return p; }
 
 // per-seed reduction of up to K values; op 0 = sum, 1 = min, 2 = max. Result in c.out[k*MAXG + sg].
 template <int K>
@@ -188,24 +201,6 @@ __device__ __forceinline__ double lanes_sum(const Ctx &c, double a)
     return a;
 }
 
-// y = alpha * (M x) [+ y0]  row-wise CSR; M values Mv group-blocked
-// (chunked variants with four entries in flight are slower: inside the solver body the 64-register budget of a
-// 1024-thread CTA spills them)
-__device__ __forceinline__ double row_dot(const int *rp, const int *ci, const double *Mv, const double *x, int r,
-                                          int G, int sg)
-{
-    double acc = 0.0;
-    for (int k = rp[r]; k < rp[r + 1]; k++) acc = fma(Mv[GI(k)], x[GI(ci[k])], acc);
-    return acc;
-}
-// (M' y)_v via the transposed pattern with value map
-__device__ __forceinline__ double col_dot(const int *trp, const int *tri, const int *tvi, const double *Mv,
-                                          const double *y, int v, int G, int sg)
-{
-    double acc = 0.0;
-    for (int k = trp[v]; k < trp[v + 1]; k++) acc = fma(Mv[GI(tvi[k])], y[GI(tri[k])], acc);
-    return acc;
-}
 
 // ---- cone operators (one thread per LP row / per SOC cone, per seed) ----
 // out = W^-2 * in
@@ -530,19 +525,20 @@ __device__ __noinline__ void kkt_sweep_sn(const SnArgs *ap, int tid)
     }
 }
 
-__device__ __forceinline__ void kkt_ldl_solve_sn(const IpmProgram &P, Ctx &c, const double *invD, double *v)
+// (L D L') v = v for v = ipm_ar.rhs
+__device__ __forceinline__ void kkt_ldl_solve_sn(const IpmProgram &P, Ctx &c)
 {
     const int G = c.G, sg = c.sg;
-    double *vs = c.vs;
+    const IpmGroup &ar = ipm_ar;
     IPM_STAMP(15)
-    for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
+    for (int i = c.slot; i < P.nk; i += c.nslots) ar.vs[i * G + sg] = glb(ar.rhs)[GI(i)];
     __syncthreads();
     kkt_sweep_sn<1>(c.s_sn, c.tid);
     if (c.tid == 0) { const long long t1_ = clock64(); ipm_s_prof[8] += t1_ - ipm_s_prof[15]; ipm_s_prof[15] = t1_; }
-    for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] *= invD[GI(i)];
+    for (int i = c.slot; i < P.nk; i += c.nslots) ar.vs[i * G + sg] *= glb(ar.invD)[GI(i)];
     __syncthreads();
     kkt_sweep_sn<-1>(c.s_sn, c.tid);
-    for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] = vs[i * G + sg];
+    for (int i = c.slot; i < P.nk; i += c.nslots) glb(ar.rhs)[GI(i)] = ar.vs[i * G + sg];
     __syncthreads();
     if (c.tid == 0) { ipm_s_prof[9] += clock64() - ipm_s_prof[15]; ipm_s_prof[10] += 1; }
 }
@@ -724,35 +720,37 @@ __device__ __noinline__ void solve_sweep()
 }
 
 template <int SN>
-__device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c, const double *Ls, const double *invD, double *v)
+__device__ __forceinline__ void kkt_ldl_solve_smem(const IpmProgram &P, Ctx &c)
 {
     const int G = c.G, sg = c.sg;
-    double *vs = c.vs;
+    const IpmGroup &ar = ipm_ar;
     IPM_STAMP(15)
-    for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] = v[GI(i)];
+    for (int i = c.slot; i < P.nk; i += c.nslots) ar.vs[i * G + sg] = glb(ar.rhs)[GI(i)];
     // forward (level 0 rows are empty: leaves have no dependencies); the barrier inside the sweep publishes vs
     solve_sweep<1>();
     if (P.nlevels <= 1) __syncthreads();
     if constexpr (SN == 2) kkt_sweep_top<1>(c.s_hy, c.tid);   // after the bridge level: column-oriented top panels
     if (c.tid == 0) { const long long t1_ = clock64(); ipm_s_prof[8] += t1_ - ipm_s_prof[15]; ipm_s_prof[15] = t1_; }
-    for (int i = c.slot; i < P.nk; i += c.nslots) vs[i * G + sg] *= invD[GI(i)];
+    for (int i = c.slot; i < P.nk; i += c.nslots) ar.vs[i * G + sg] *= glb(ar.invD)[GI(i)];
     if constexpr (SN == 2) { __syncthreads(); kkt_sweep_top<-1>(c.s_hy, c.tid); }
     // backward (the top level holds roots only: empty columns)
     solve_sweep<-1>();
     if (P.nlevels <= 1) __syncthreads();
-    for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] = vs[i * G + sg];
+    for (int i = c.slot; i < P.nk; i += c.nslots) glb(ar.rhs)[GI(i)] = ar.vs[i * G + sg];
     __syncthreads();
     if (c.tid == 0) { ipm_s_prof[9] += clock64() - ipm_s_prof[15]; ipm_s_prof[10] += 1; }
 }
 
-// in-place solve of (L D L') v = rhs on the permuted vector v
+// in-place solve of (L D L') v = rhs on the permuted vector v = ipm_ar.rhs
 template <int SN>
-__device__ __forceinline__ void kkt_ldl_solve(const IpmProgram &P, Ctx &c, const double *Ls, const double *invD, double *v)
+__device__ __forceinline__ void kkt_ldl_solve(const IpmProgram &P, Ctx &c)
 {
-    if constexpr (SN == 1) { kkt_ldl_solve_sn(P, c, invD, v); return; }
-    if (SN == 2 || c.vs) { kkt_ldl_solve_smem<SN>(P, c, Ls, invD, v); return; }
+    if constexpr (SN == 1) { kkt_ldl_solve_sn(P, c); return; }
+    if (SN == 2 || ipm_ar.vs) { kkt_ldl_solve_smem<SN>(P, c); return; }
     set_lanes(c, c.Rmax);
     const int G = c.G, sg = c.sg;
+    const double *Ls = glb(ipm_ar.Ls);
+    double *v = glb(ipm_ar.rhs);
     for (int lv = 0; lv < P.nlevels; lv++) {   // forward, rows of L
         const int wend = c.s_lvl[lv + 1];
         for (int w0 = c.s_lvl[lv]; w0 < wend; w0 += c.nisl) {
@@ -778,7 +776,7 @@ __device__ __forceinline__ void kkt_ldl_solve(const IpmProgram &P, Ctx &c, const
         }
         __syncthreads();
     }
-    for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] *= invD[GI(i)];
+    for (int i = c.slot; i < P.nk; i += c.nslots) v[GI(i)] *= glb(ipm_ar.invD)[GI(i)];
     __syncthreads();
     for (int lv = P.nlevels - 1; lv >= 0; lv--) {   // backward, columns of L
         const int wend = c.s_lvl[lv + 1];
@@ -807,80 +805,232 @@ __device__ __forceinline__ void kkt_ldl_solve(const IpmProgram &P, Ctx &c, const
     }
 }
 
+// ---- sparse products of the residuals and of kkt_solve ------------------------------------------------------------
+// Row r of M x is one thread's sequential fma chain from 0.0 over the row's entries in order, and so is a column of a
+// transposed product M'y (through the transposed pattern and its value map); composite expressions keep their order,
+// e.g. (c + A'y) + G'z.  A thread issues the index loads, then the value and operand gathers, of up to IPM_PF entries of
+// its row at once, and requests the extent of its next row while the current one is in flight.  The products are
+// separate (noinline) functions whose arguments come from shared memory (ipm_mv, ipm_ar), like the level programs:
+// inlined in the solver body, rows with several entries in flight do not fit the registers of a 1024-thread CTA and are
+// spilled.  G is a compile-time constant (one inlined copy per group size behind each entry point).
+struct SpmvArgs {   // CTA-uniform: one block per launch in shared memory
+    const int *A_rp, *A_ci, *G_rp, *G_ci;
+    const int *At_rp, *At_ri, *At_vi, *Gt_rp, *Gt_ri, *Gt_vi;
+    const int *iperm;
+    int n, p, m, G;
+    const double *by, *bz;   // operands of the current kkt_solve, written by thread 0 when it starts
+    double *dx, *dy, *dz;
+};
+__shared__ SpmvArgs ipm_mv;
+
+// sum of Mv[vi(k)] * x[ci(k)] over k in [k0, k1) in k order; T: vi is the value map of a transposed pattern, else vi(k) = k
+template <int G, bool T>
+__device__ __forceinline__ double spmv_dot(const int *ci, const int *vi, const double *Mv, const double *x, int k0, int k1)
+{
+    const int sg = threadIdx.x & (G - 1);
+    __builtin_assume(__isGlobal(ci)); __builtin_assume(__isGlobal(Mv)); __builtin_assume(__isGlobal(x));
+    if (T) __builtin_assume(__isGlobal(vi));
+    double acc = 0.0;
+    for (int k = k0; k < k1; k += IPM_PF) {
+        int xi[IPM_PF], mi[IPM_PF];
+#pragma unroll
+        for (int j = 0; j < IPM_PF; j++) {
+            const bool on = k + j < k1;
+            xi[j] = on ? ci[k + j] : 0;
+            mi[j] = on ? (T ? vi[k + j] : k + j) : 0;
+        }
+        double mv[IPM_PF], xv[IPM_PF];
+#pragma unroll
+        for (int j = 0; j < IPM_PF; j++) {
+            const bool on = k + j < k1;
+            mv[j] = on ? Mv[mi[j] * G + sg] : 0.0;
+            xv[j] = on ? x[xi[j] * G + sg] : 0.0;
+        }
+#pragma unroll
+        for (int j = 0; j < IPM_PF; j++)
+            if (k + j < k1) acc = fma(mv[j], xv[j], acc);   // skipped, not fma(0, 0, acc): that would turn -0 into +0
+    }
+    return acc;
+}
+// f(r, (M x)_r) for this thread's rows r = slot, slot + nslots, ... < nrows
+template <int G, bool T, class F>
+__device__ __forceinline__ void spmv_rows(const int *rp, const int *ci, const int *vi, const double *Mv, const double *x,
+                                          int nrows, F &&f)
+{
+    __builtin_assume(__isGlobal(rp));
+    const int nslots = blockDim.x / G;
+    int r = threadIdx.x / G, k0 = 0, k1 = 0;
+    if (r < nrows) { k0 = rp[r]; k1 = rp[r + 1]; }
+    for (; r < nrows; r += nslots) {
+        const int c0 = k0, c1 = k1;
+        if (r + nslots < nrows) { k0 = rp[r + nslots]; k1 = rp[r + nslots + 1]; }
+        f(r, spmv_dot<G, T>(ci, vi, Mv, x, c0, c1));
+    }
+}
+// f(v, (M1' x1)_v, (M2' x2)_v) for this thread's columns v < ncols of two transposed products
+template <int G, class F>
+__device__ __forceinline__ void spmv_cols2(const int *rp1, const int *ri1, const int *vi1, const double *M1, const double *x1,
+                                           const int *rp2, const int *ri2, const int *vi2, const double *M2, const double *x2,
+                                           int ncols, F &&f)
+{
+    __builtin_assume(__isGlobal(rp1)); __builtin_assume(__isGlobal(rp2));
+    const int nslots = blockDim.x / G;
+    int v = threadIdx.x / G, k0 = 0, k1 = 0, l0 = 0, l1 = 0;
+    if (v < ncols) { k0 = rp1[v]; k1 = rp1[v + 1]; l0 = rp2[v]; l1 = rp2[v + 1]; }
+    for (; v < ncols; v += nslots) {
+        const int c0 = k0, c1 = k1, d0 = l0, d1 = l1;
+        if (v + nslots < ncols) { k0 = rp1[v + nslots]; k1 = rp1[v + nslots + 1]; l0 = rp2[v + nslots]; l1 = rp2[v + nslots + 1]; }
+        const double a1 = spmv_dot<G, true>(ri1, vi1, M1, x1, c0, c1);
+        f(v, a1, spmv_dot<G, true>(ri2, vi2, M2, x2, d0, d1));
+    }
+}
+#define IPM_G_DISPATCH(F)                                                                 \
+    switch (ipm_mv.G) {                                                                   \
+        case 1: return F<1>();                                                            \
+        case 2: return F<2>();                                                            \
+        case 4: return F<4>();                                                            \
+        default: return F<8>();                                                           \
+    }
+
+// residuals: rx = (c + A'y) + G'z, ry = Ax - b, rz = (Gx + s) - h
+template <int G>
+__device__ __forceinline__ void spmv_residuals_g()
+{
+    const SpmvArgs &a = ipm_mv;
+    const IpmGroup &ar = ipm_ar;
+    const int sg = threadIdx.x & (G - 1);
+    spmv_cols2<G>(a.At_rp, a.At_ri, a.At_vi, glb(ar.Av), glb(ar.y), a.Gt_rp, a.Gt_ri, a.Gt_vi, glb(ar.Gv), glb(ar.z), a.n,
+                  [&](int i, double ay, double gz) { glb(ar.rx)[i * G + sg] = glb(ar.cc)[i * G + sg] + ay + gz; });
+    spmv_rows<G, false>(a.A_rp, a.A_ci, nullptr, glb(ar.Av), glb(ar.x), a.p,
+                        [&](int i, double ax) { glb(ar.ry)[i * G + sg] = ax - glb(ar.bb)[i * G + sg]; });
+    spmv_rows<G, false>(a.G_rp, a.G_ci, nullptr, glb(ar.Gv), glb(ar.x), a.m,
+                        [&](int i, double gx) { glb(ar.rz)[i * G + sg] = gx + glb(ar.s)[i * G + sg] - glb(ar.hh)[i * G + sg]; });
+}
+__device__ __noinline__ void spmv_residuals() { IPM_G_DISPATCH(spmv_residuals_g) }
+
+// right-hand side of the reduced system: r1 = r1 + G'tm, rhs = r1 (permuted), dx = 0
+template <int G>
+__device__ __forceinline__ void spmv_kkt_rhs_g()
+{
+    const SpmvArgs &a = ipm_mv;
+    const IpmGroup &ar = ipm_ar;
+    const int sg = threadIdx.x & (G - 1);
+    spmv_rows<G, true>(a.Gt_rp, a.Gt_ri, a.Gt_vi, glb(ar.Gv), glb(ar.tm), a.n, [&](int v, double gt) {
+        const double r = glb(ar.r1)[v * G + sg] + gt;
+        glb(ar.r1)[v * G + sg] = r;
+        glb(ar.rhs)[glb(a.iperm)[v] * G + sg] = r;
+        glb(a.dx)[v * G + sg] = 0.0;
+    });
+}
+__device__ __noinline__ void spmv_kkt_rhs() { IPM_G_DISPATCH(spmv_kkt_rhs_g) }
+
+// gm = G dx, or G dx - bz
+template <bool BZ, int G>
+__device__ __forceinline__ void spmv_kkt_gdx_g()
+{
+    const SpmvArgs &a = ipm_mv;
+    const IpmGroup &ar = ipm_ar;
+    const int sg = threadIdx.x & (G - 1);
+    spmv_rows<G, false>(a.G_rp, a.G_ci, nullptr, glb(ar.Gv), glb(a.dx), a.m,
+                        [&](int r, double gx) { glb(ar.gm)[r * G + sg] = BZ ? gx - glb(a.bz)[r * G + sg] : gx; });
+}
+template <int G> __device__ __forceinline__ void spmv_kkt_gdx_g0() { spmv_kkt_gdx_g<false, G>(); }
+template <int G> __device__ __forceinline__ void spmv_kkt_gdx_g1() { spmv_kkt_gdx_g<true, G>(); }
+template <bool BZ>
+__device__ __noinline__ void spmv_kkt_gdx()
+{
+    if constexpr (BZ) { IPM_G_DISPATCH(spmv_kkt_gdx_g1) } else { IPM_G_DISPATCH(spmv_kkt_gdx_g0) }
+}
+
+// residual of the reduced system into rhs (permuted): r1 - G'e1 - A'dy (e1 = W^-2 G dx) and by - A dx.  Returns this
+// thread's |residual|_inf and |r1, by|_inf; a NaN entry counts as +inf (fmax would drop it)
+template <int G>
+__device__ __forceinline__ double2 spmv_kkt_refine_g()
+{
+    const SpmvArgs &a = ipm_mv;
+    const IpmGroup &ar = ipm_ar;
+    const int sg = threadIdx.x & (G - 1);
+    double n0 = 0.0, n1 = 0.0;
+    spmv_cols2<G>(a.Gt_rp, a.Gt_ri, a.Gt_vi, glb(ar.Gv), glb(ar.e1), a.At_rp, a.At_ri, a.At_vi, glb(ar.Av), glb(a.dy), a.n,
+                  [&](int v, double ge, double ay) {
+                      const double bx = glb(ar.r1)[v * G + sg];
+                      const double r = bx - ge - ay;
+                      glb(ar.rhs)[glb(a.iperm)[v] * G + sg] = r;
+                      n0 = fmax(n0, r == r ? fabs(r) : CUDART_INF); n1 = fmax(n1, fabs(bx));
+                  });
+    spmv_rows<G, false>(a.A_rp, a.A_ci, nullptr, glb(ar.Av), glb(a.dx), a.p, [&](int r, double ax) {
+        const double by = glb(a.by)[r * G + sg];
+        const double rr = by - ax;
+        glb(ar.rhs)[glb(a.iperm)[a.n + r] * G + sg] = rr;
+        n0 = fmax(n0, rr == rr ? fabs(rr) : CUDART_INF); n1 = fmax(n1, fabs(by));
+    });
+    return make_double2(n0, n1);
+}
+__device__ __noinline__ double2 spmv_kkt_refine() { IPM_G_DISPATCH(spmv_kkt_refine_g) }
+#undef IPM_G_DISPATCH
+
 // Solve [0 A' G'; A 0 0; G 0 -W'W][dx;dy;dz] = [bx;by;bz] through the reduced system
 //   (G' W^-2 G) dx + A' dy = bx + G' W^-2 bz ,  A dx = by ,  dz = W^-2 (G dx - bz)
 // with nref steps of iterative refinement against the unregularised reduced operator.
-// bx,by,bz are overwritten/consumed: bx -> r1 (in place), by -> r2 (kept), bz kept.
+// bx is r1, overwritten by bx + G' W^-2 bz; by and bz are kept.  Leaves G dx - bz in gm.
 template <int SN>
-__device__ __forceinline__ void kkt_solve(const IpmProgram &P, Ctx &c, const IpmData &D, const double *Av, const double *Gv,
-                          const double *wm, const double *socw, const double *soceta, double *bx, const double *by,
-                          const double *bz, double *dx, double *dy, double *dz, double *tm, double *gm, double *e1,
-                          double *e2, double *rhs, const double *Ls, const double *invD, int nref)
+__device__ __forceinline__ void kkt_solve(const IpmProgram &P, Ctx &c, const double *by, const double *bz, double *dx,
+                                          double *dy, double *dz, int nref)
 {
     const int G = c.G, sg = c.sg;
-    // tm = W^-2 bz ; r1 = bx + G' tm
-    apply_winv2(P, c, wm, socw, soceta, bz, tm);
+    const IpmGroup &ar = ipm_ar;
+    const SpmvArgs &a = ipm_mv;
+    if (c.tid == 0) { ipm_mv.by = by; ipm_mv.bz = bz; ipm_mv.dx = dx; ipm_mv.dy = dy; ipm_mv.dz = dz; }
+    // tm = W^-2 bz ; r1 = bx + G' tm  (the barrier publishes the operands too)
+    apply_winv2(P, c, glb(ar.wm), glb(ar.socw), glb(ar.soceta), bz, glb(ar.tm));
     __syncthreads();
-    for (int v = c.slot; v < P.n; v += c.nslots) {
-        const double r = bx[GI(v)] + col_dot(P.Gt_rp, P.Gt_ri, P.Gt_vi, Gv, tm, v, G, sg);
-        bx[GI(v)] = r;
-        rhs[GI(P.iperm[v])] = r;
-        dx[GI(v)] = 0.0;
-    }
-    for (int r = c.slot; r < P.p; r += c.nslots) { rhs[GI(P.iperm[P.n + r])] = by[GI(r)]; dy[GI(r)] = 0.0; }
+    spmv_kkt_rhs();
+    for (int r = c.slot; r < P.p; r += c.nslots) { glb(ar.rhs)[GI(P.iperm[P.n + r])] = glb(a.by)[GI(r)]; glb(a.dy)[GI(r)] = 0.0; }
     __syncthreads();
+    int again = 1;   // 0: the refinement loop ended on its residual check
     for (int it = 0;; it++) {
-        kkt_ldl_solve<SN>(P, c, Ls, invD, rhs);
-        for (int v = c.slot; v < P.n; v += c.nslots) dx[GI(v)] += rhs[GI(P.iperm[v])];
-        for (int r = c.slot; r < P.p; r += c.nslots) dy[GI(r)] += rhs[GI(P.iperm[P.n + r])];
+        kkt_ldl_solve<SN>(P, c);
+        for (int v = c.slot; v < P.n; v += c.nslots) glb(a.dx)[GI(v)] += glb(ar.rhs)[GI(P.iperm[v])];
+        for (int r = c.slot; r < P.p; r += c.nslots) glb(a.dy)[GI(r)] += glb(ar.rhs)[GI(P.iperm[P.n + r])];
         __syncthreads();
         if (it >= nref) break;
         // residual of the reduced system: e1 = r1 - (G' W^-2 G dx + A' dy), e2 = by - A dx
-        for (int r = c.slot; r < P.m; r += c.nslots) gm[GI(r)] = row_dot(P.G_rp, P.G_ci, Gv, dx, r, G, sg);
+        spmv_kkt_gdx<false>();
         __syncthreads();
-        apply_winv2(P, c, wm, socw, soceta, gm, e1);  // e1: max(n,m)-sized scratch holding W^-2 G dx
+        apply_winv2(P, c, glb(ar.wm), glb(ar.socw), glb(ar.soceta), glb(ar.gm), glb(ar.e1));  // e1: max(n,m)-sized scratch holding W^-2 G dx
         __syncthreads();
-        // |residual|_inf, |rhs|_inf; a NaN entry counts as +inf (fmax would drop it)
-        double nrm[2] = {0.0, 0.0};
-        for (int v = c.slot; v < P.n; v += c.nslots) {
-            const double r = bx[GI(v)] - col_dot(P.Gt_rp, P.Gt_ri, P.Gt_vi, Gv, e1, v, G, sg) -
-                             col_dot(P.At_rp, P.At_ri, P.At_vi, Av, dy, v, G, sg);
-            rhs[GI(P.iperm[v])] = r;
-            nrm[0] = fmax(nrm[0], r == r ? fabs(r) : CUDART_INF); nrm[1] = fmax(nrm[1], fabs(bx[GI(v)]));
-        }
-        for (int r = c.slot; r < P.p; r += c.nslots) {
-            const double rr = by[GI(r)] - row_dot(P.A_rp, P.A_ci, Av, dx, r, G, sg);
-            rhs[GI(P.iperm[P.n + r])] = rr;
-            nrm[0] = fmax(nrm[0], rr == rr ? fabs(rr) : CUDART_INF); nrm[1] = fmax(nrm[1], fabs(by[GI(r)]));
-        }
+        // |residual|_inf, |rhs|_inf
+        const double2 n_ = spmv_kkt_refine();
+        double nrm[2] = {n_.x, n_.y};
         seed_reduce<2>(c, nrm, 2);   // ends with a barrier: rhs is complete as well
         if (c.tid == 0) {
             // the group refines again while one of its seeds asks for it.  Finished seeds (converged, failed, skipped by
             // the caller, padded lanes) have no vote: their directions are not used.  Nor has a seed whose residual is
             // not finite: refining cannot repair it, and its next residual check ends it as NUMERICAL.  Without these
             // exclusions a seed's bits depended on whether its group was padded or held a NaN seed.
-            int again = 0;
+            int again_ = 0;
             for (int q = 0; q < G; q++) {
                 const double res = c.out[q], ref = c.out[IPM_MAXG + q];
                 if (c.s_done[q] || !isfinite(res)) continue;
                 // early iterations only need a direction; the last ones (small mu: the scaling matrix spans > 20 orders of
                 // magnitude) need every digit, or the iterates stall a decade or two above the requested gap
-                const double tol_ = (c.s_mu[q] > c.mu_tight) ? c.reftol : fmin(c.reftol, 1e-13);
-                if (!(res <= tol_ * (1.0 + ref))) again = 1;
+                const double tol_ = (c.s_mu[q] > ar.mu_tight) ? ar.reftol : fmin(ar.reftol, 1e-13);
+                if (!(res <= tol_ * (1.0 + ref))) again_ = 1;
             }
-            *c.flag = again;
+            *c.flag = again_;
         }
         __syncthreads();
-        const int again = *c.flag;
+        again = *c.flag;
         __syncthreads();
         if (!again) break;
     }
-    // dz = W^-2 (G dx - bz)
-    for (int r = c.slot; r < P.m; r += c.nslots) gm[GI(r)] = row_dot(P.G_rp, P.G_ci, Gv, dx, r, G, sg) - bz[GI(r)];
+    // dz = W^-2 (G dx - bz).  After a residual check that ended the loop, gm already holds G dx of the final dx (the
+    // subtraction follows the full row sum either way: the same bits)
+    if (again) spmv_kkt_gdx<true>();
+    else for (int r = c.slot; r < P.m; r += c.nslots) glb(ar.gm)[GI(r)] -= glb(a.bz)[GI(r)];
     __syncthreads();
-    apply_winv2(P, c, wm, socw, soceta, gm, dz);
+    apply_winv2(P, c, glb(ar.wm), glb(ar.socw), glb(ar.soceta), glb(ar.gm), glb(a.dz));
     __syncthreads();
-    (void)e2; (void)D;
 }
 
 // smallest t with u + t e in K  (max over cones); thread-partial, to be max-reduced
@@ -1151,9 +1301,8 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
     c.o_fal = nl1; c.o_fbl = 2 * nl1; c.o_faR = 4 * nl1;
     c.o_fwl = 5 * nl1; c.o_bwl = 6 * nl1; c.o_fwR = 7 * nl1; c.o_bwR = 8 * nl1;
     c.o_vs = (9 * (P.nlevels + 1) + 3) & ~3;
-    c.vs = D.vsmem ? (double *)(s_lv + c.o_vs) : nullptr;
     c.G = D.G; c.tid = threadIdx.x; c.sg = c.tid % c.G; c.slot = c.tid / c.G; c.nslots = NT / c.G; c.nwarps = NT / 32;
-    c.flag = &s_flag; c.reftol = O.reftol; c.s_mu = s_mu; c.mu_tight = O.mu_tight;
+    c.flag = &s_flag; c.s_mu = s_mu;
     c.Rmax = D.R;
     c.lprof = (blockIdx.x == 0 && threadIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 : nullptr;
     if (c.lprof) for (int i = 0; i < 3 * (P.nlevels + (SN == 2 ? P.hy.ntl : 0)); i++) c.lprof[i] = 0;
@@ -1166,69 +1315,83 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
     const bool live = seed < D.B;  // padded seeds replicate work harmlessly (arrays are padded)
     (void)live;
 
-#define GP(arr, E) ((arr) + g * (size_t)(E) * G)
-    double *Av = GP(D.Av, P.nnzA), *Gv = GP(D.Gv, P.nnzG), *cc = GP(D.c, P.n), *bb = GP(D.b, P.p), *hh = GP(D.h, P.m);
-    double *eqD = GP(D.eqD, P.n), *eqA = GP(D.eqA, P.p), *eqG = GP(D.eqG, P.m);
-    double *x = GP(D.x, P.n), *y = GP(D.y, P.p), *z = GP(D.z, P.m), *s = GP(D.s, P.m);
-    double *xb = GP(D.xb, P.n), *yb = GP(D.yb, P.p), *zb = GP(D.zb, P.m), *sb = GP(D.sb, P.m);
-    double *rx = GP(D.rx, P.n), *ry = GP(D.ry, P.p), *rz = GP(D.rz, P.m), *lam = GP(D.lam, P.m);
-    double *wm = GP(D.wm, P.nwm), *socw = GP(D.socw, P.m - P.l + 1), *soceta = GP(D.soceta, P.nsoc + 1);
-    double *dx = GP(D.dx, P.n), *dy = GP(D.dy, P.p), *dz = GP(D.dz, P.m), *ds = GP(D.ds, P.m);
-    double *dsa = GP(D.dsa, P.m), *dza = GP(D.dza, P.m), *tm = GP(D.tm, P.m), *gm = GP(D.gm, P.m);
-    double *r1 = GP(D.r1, P.n), *r2 = GP(D.r2, P.p);
-    const int nm = (P.n > P.m ? P.n : P.m);
-    double *e1 = GP(D.e1, nm), *e2 = GP(D.e2, P.p), *rhs = GP(D.rhs, P.nk);
-    double *Y = GP(D.Y, P.ysize), *Ls = GP(D.Ls, P.nnzL + 1), *invD = GP(D.invD, P.nk);
-    c.sn = D.sn; c.Ypanels = Y; c.ysize = (size_t)P.ysize;
-    c.s_done = s_done; c.s_delta = s_delta; c.s_bad = s_bad; c.rho_min = O.rho_min; c.bad_abs = O.bad_abs;
-    if (threadIdx.x == 0) { ipm_s_reg[0] = O.rho_min; ipm_s_reg[1] = O.bad_abs; }
+    c.s_done = s_done; c.s_delta = s_delta; c.s_bad = s_bad;
+    c.sn = D.sn; c.ysize = (size_t)P.ysize;
     c.s_sn = &s_snargs;
     c.s_hy = &s_hyargs;
-    if (SN == 2 && threadIdx.x == 0) {
-        HyArgs a;
-        a.hy = P.hy; a.Y = Y; a.Ls = Ls; a.invD = invD; a.s_done = s_done; a.s_delta = s_delta; a.s_bad = s_bad;
-        a.rho_min = O.rho_min; a.bad_abs = O.bad_abs; a.o_vs = c.o_vs; a.nnzL = P.nnzL; a.G = D.G; a.nwarps = NT / 32;
-        a.lprof = (blockIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 + 3 * P.nlevels : nullptr;
-        s_hyargs = a;
-    }
-    if (SN == 1 && threadIdx.x == 0) {
-        SnArgs a;
-        a.sn = P.sn; a.Y = Y; a.invD = invD; a.vs = c.vs; a.s_done = s_done; a.s_delta = s_delta; a.s_bad = s_bad;
-        a.rho_min = O.rho_min; a.bad_abs = O.bad_abs; a.ysize = (size_t)P.ysize; a.G = D.G; a.tid = 0; a.nwarps = NT / 32;
-        a.nls = P.nlevels; a.lprof = (blockIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 : nullptr;
-        s_snargs = a;
-    }
-    c.Lrow = GP(D.Lrow, P.nnzL + 1);
-    if (D.psmem) {   // dynamic window: level pointers | vector, or the factorisation's slots | substitution slots | counters
-        const int vw = 2 * (P.nk > P.npf ? P.nk : P.npf) * G;
-        c.fpart = (double *)(s_lv + c.o_vs);
-        c.spart = (double *)(s_lv + c.o_vs + vw);
-        c.pcnt = (unsigned *)(s_lv + c.o_vs + vw + 2 * P.nps * G);
-        for (int i = c.tid; i < P.nps * G; i += NT) c.pcnt[i] = 0u;   // the barrier below publishes it
-    } else {
-        c.fpart = c.spart = GP(D.part, P.npart + 1);
-        c.pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
-    }
-    if (SN != 1 && threadIdx.x == 0) {
-        FactorArgs a;
-        a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fb_cmb = P.fb_cmb;
-        a.Y = Y; a.Ls = Ls; a.Lrow = c.Lrow; a.invD = invD; a.part = c.fpart;
-        a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
-        a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = G; a.nslots = c.nslots;
-        a.lprof = c.lprof;   // thread 0 of CTA 0 only (c.lprof is nullptr everywhere else)
-        ipm_fa = a;
-        SweepArgs w;
-        w.nl = P.nlevels; w.G = G; w.nslots = c.nslots; w.o_vs = c.o_vs; w.part = c.spart; w.pcnt = c.pcnt;
-        w.items = P.fwp_item; w.idxarr = P.Lr_col; w.vals = c.Lrow; w.o_lvl = c.o_fwl; w.o_R = c.o_fwR; w.lv0 = 1;
-        w.cmb = P.fwc_item;
-        w.lprof = c.lprof ? c.lprof + P.nlevels : nullptr;
-        ipm_sw[0] = w;
-        w.items = P.bwp_item; w.idxarr = P.L_ri; w.vals = Ls; w.o_lvl = c.o_bwl; w.o_R = c.o_bwR; w.lv0 = P.nlevels - 2;
-        w.cmb = P.bwc_item;
-        w.lprof = c.lprof ? c.lprof + 2 * P.nlevels : nullptr;
-        ipm_sw[1] = w;
-    }
+    double *const vs = D.vsmem ? (double *)(s_lv + c.o_vs) : nullptr;
+    unsigned *const pcnt_s = (unsigned *)(s_lv + c.o_vs + 2 * (P.nk > P.npf ? P.nk : P.npf) * G + 2 * P.nps * G);
+    if (D.psmem) for (int i = c.tid; i < P.nps * G; i += NT) pcnt_s[i] = 0u;   // the barrier below publishes it
+    if (threadIdx.x == 0) {   // the CTA-uniform argument blocks (published by the barrier below)
+        ipm_s_reg[0] = O.rho_min; ipm_s_reg[1] = O.bad_abs;
+#define GP(arr, E) ((arr) + g * (size_t)(E) * G)
+        IpmGroup r;
+        r.Av = GP(D.Av, P.nnzA); r.Gv = GP(D.Gv, P.nnzG); r.cc = GP(D.c, P.n); r.bb = GP(D.b, P.p); r.hh = GP(D.h, P.m);
+        r.eqD = GP(D.eqD, P.n); r.eqA = GP(D.eqA, P.p); r.eqG = GP(D.eqG, P.m);
+        r.x = GP(D.x, P.n); r.y = GP(D.y, P.p); r.z = GP(D.z, P.m); r.s = GP(D.s, P.m);
+        r.xb = GP(D.xb, P.n); r.yb = GP(D.yb, P.p); r.zb = GP(D.zb, P.m); r.sb = GP(D.sb, P.m);
+        r.rx = GP(D.rx, P.n); r.ry = GP(D.ry, P.p); r.rz = GP(D.rz, P.m); r.lam = GP(D.lam, P.m);
+        r.wm = GP(D.wm, P.nwm); r.socw = GP(D.socw, P.m - P.l + 1); r.soceta = GP(D.soceta, P.nsoc + 1);
+        r.dx = GP(D.dx, P.n); r.dy = GP(D.dy, P.p); r.dz = GP(D.dz, P.m); r.ds = GP(D.ds, P.m);
+        r.dsa = GP(D.dsa, P.m); r.dza = GP(D.dza, P.m); r.tm = GP(D.tm, P.m); r.gm = GP(D.gm, P.m);
+        r.r1 = GP(D.r1, P.n); r.r2 = GP(D.r2, P.p);
+        r.e1 = GP(D.e1, (P.n > P.m ? P.n : P.m)); r.rhs = GP(D.rhs, P.nk);
+        r.Y = GP(D.Y, P.ysize); r.Ls = GP(D.Ls, P.nnzL + 1); r.invD = GP(D.invD, P.nk);
+        r.vs = vs; r.reftol = O.reftol; r.mu_tight = O.mu_tight;
+        ipm_ar = r;
+        SpmvArgs m;
+        m.A_rp = P.A_rp; m.A_ci = P.A_ci; m.G_rp = P.G_rp; m.G_ci = P.G_ci;
+        m.At_rp = P.At_rp; m.At_ri = P.At_ri; m.At_vi = P.At_vi; m.Gt_rp = P.Gt_rp; m.Gt_ri = P.Gt_ri; m.Gt_vi = P.Gt_vi;
+        m.iperm = P.iperm; m.n = P.n; m.p = P.p; m.m = P.m; m.G = G;
+        ipm_mv = m;
+        if (SN == 2) {
+            HyArgs a;
+            a.hy = P.hy; a.Y = r.Y; a.Ls = r.Ls; a.invD = r.invD; a.s_done = s_done; a.s_delta = s_delta; a.s_bad = s_bad;
+            a.rho_min = O.rho_min; a.bad_abs = O.bad_abs; a.o_vs = c.o_vs; a.nnzL = P.nnzL; a.G = D.G; a.nwarps = NT / 32;
+            a.lprof = (blockIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 + 3 * P.nlevels : nullptr;
+            s_hyargs = a;
+        }
+        if (SN == 1) {
+            SnArgs a;
+            a.sn = P.sn; a.Y = r.Y; a.invD = r.invD; a.vs = vs; a.s_done = s_done; a.s_delta = s_delta; a.s_bad = s_bad;
+            a.rho_min = O.rho_min; a.bad_abs = O.bad_abs; a.ysize = (size_t)P.ysize; a.G = D.G; a.tid = 0; a.nwarps = NT / 32;
+            a.nls = P.nlevels; a.lprof = (blockIdx.x == 0 && D.prof && D.lvl_prof) ? D.prof + 12 : nullptr;
+            s_snargs = a;
+        }
+        if (SN != 1) {
+            // partial sums of the split targets of a level: in the dynamic window (level pointers | vector, or the
+            // factorisation's slots | substitution slots | counters), or in global memory
+            double *Lrow = GP(D.Lrow, P.nnzL + 1), *fpart, *spart;
+            unsigned *pcnt;
+            if (D.psmem) {
+                fpart = (double *)(s_lv + c.o_vs);
+                spart = (double *)(s_lv + c.o_vs + 2 * (P.nk > P.npf ? P.nk : P.npf) * G);
+                pcnt = pcnt_s;
+            } else {
+                fpart = spart = GP(D.part, P.npart + 1);
+                pcnt = (unsigned *)GP(D.pcnt, P.npart + 1);
+            }
+            FactorArgs a;
+            a.fa_item = P.fa_item; a.fb_item = P.fb_item; a.ft_op = P.ft_op; a.fb_cmb = P.fb_cmb;
+            a.Y = r.Y; a.Ls = r.Ls; a.Lrow = Lrow; a.invD = r.invD; a.part = fpart;
+            a.o_fal = c.o_fal; a.o_faR = c.o_faR; a.o_fbl = c.o_fbl;
+            a.nl = P.nlevels; a.nnzLd = P.nnzL; a.G = G; a.nslots = c.nslots;
+            a.lprof = c.lprof;   // thread 0 of CTA 0 only (c.lprof is nullptr everywhere else)
+            ipm_fa = a;
+            SweepArgs w;
+            w.nl = P.nlevels; w.G = G; w.nslots = c.nslots; w.o_vs = c.o_vs; w.part = spart; w.pcnt = pcnt;
+            w.items = P.fwp_item; w.idxarr = P.Lr_col; w.vals = Lrow; w.o_lvl = c.o_fwl; w.o_R = c.o_fwR; w.lv0 = 1;
+            w.cmb = P.fwc_item;
+            w.lprof = c.lprof ? c.lprof + P.nlevels : nullptr;
+            ipm_sw[0] = w;
+            w.items = P.bwp_item; w.idxarr = P.L_ri; w.vals = r.Ls; w.o_lvl = c.o_bwl; w.o_R = c.o_bwR; w.lv0 = P.nlevels - 2;
+            w.cmb = P.bwc_item;
+            w.lprof = c.lprof ? c.lprof + 2 * P.nlevels : nullptr;
+            ipm_sw[1] = w;
+        }
 #undef GP
+    }
+    const IpmGroup &ar = ipm_ar;
 
     if (threadIdx.x == 0) {
         for (int i = 0; i < 13; i++) ipm_s_prof[i] = 0;
@@ -1253,9 +1416,9 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         if (all) return;   // CTA-uniform: nothing to solve in this group
     }
     if (D.debug_kkt) {   // test hook: one KKT solve on the device with the caller's scaling and right-hand side
-        kkt_assemble(P, c, D, Av, Gv, wm, Y, 0.0);
+        kkt_assemble(P, c, D, glb(ar.Av), glb(ar.Gv), glb(ar.wm), glb(ar.Y), 0.0);
         kkt_factor<SN>(c);
-        kkt_ldl_solve<SN>(P, c, Ls, invD, rhs);
+        kkt_ldl_solve<SN>(P, c);
         if (c.tid < G && (int)g * G + c.tid < D.B) D.status[(int)g * G + c.tid] = s_bad[c.tid];
         return;
     }
@@ -1264,7 +1427,7 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
 #define IPM_FACTOR()                                                                               \
     for (int tr_ = 0;; tr_++) {                                                                    \
         if (c.tid < G) s_bad[c.tid] = 0;                                                           \
-        kkt_assemble(P, c, D, Av, Gv, wm, Y, 0.0);                                                 \
+        kkt_assemble(P, c, D, glb(ar.Av), glb(ar.Gv), glb(ar.wm), glb(ar.Y), 0.0);                                                 \
         kkt_factor<SN>(c);                                                                         \
         if (c.tid == 0) {                                                                          \
             int again_ = 0;                                                                        \
@@ -1280,14 +1443,14 @@ __global__ void __launch_bounds__(NT) k_ipm_solve(const IpmProgram P, const IpmD
         if (!again_ || tr_ >= 4) break;                                                            \
         if (c.tid == 0) ipm_s_prof[12]++;                                                          \
     }
-    if (O.equil > 0) equilibrate(P, c, Av, Gv, cc, bb, hh, eqD, eqA, eqG, O.equil);
+    if (O.equil > 0) equilibrate(P, c, glb(ar.Av), glb(ar.Gv), glb(ar.cc), glb(ar.bb), glb(ar.hh), glb(ar.eqD), glb(ar.eqA), glb(ar.eqG), O.equil);
     PROF(0)
     // ---- data norms ----
     {
         double v[3] = {0.0, 0.0, 0.0};
-        for (int i = c.slot; i < P.p; i += c.nslots) v[0] += bb[GI(i)] * bb[GI(i)];
-        for (int i = c.slot; i < P.m; i += c.nslots) v[1] += hh[GI(i)] * hh[GI(i)];
-        for (int i = c.slot; i < P.n; i += c.nslots) v[2] += cc[GI(i)] * cc[GI(i)];
+        for (int i = c.slot; i < P.p; i += c.nslots) v[0] += glb(ar.bb)[GI(i)] * glb(ar.bb)[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) v[1] += glb(ar.hh)[GI(i)] * glb(ar.hh)[GI(i)];
+        for (int i = c.slot; i < P.n; i += c.nslots) v[2] += glb(ar.cc)[GI(i)] * glb(ar.cc)[GI(i)];
         seed_reduce<3>(c, v, 0);
         if (c.tid < G) {
             s_nb[c.tid] = fmax(1.0, sqrt(s_out[0 * IPM_MAXG + c.tid]));
@@ -1310,19 +1473,19 @@ restart_cold:
     __syncthreads();
     if (!s_allwarm) {
         // ---- starting point (CVXOPT conelp 7.1 / ECOS init): factor with W = I ----
-        set_identity_scaling(P, c, wm, socw, soceta);
+        set_identity_scaling(P, c, glb(ar.wm), glb(ar.socw), glb(ar.soceta));
         __syncthreads();
         IPM_FACTOR()
         // solve 1: [0;b;h] -> x, s = h - G x
-        for (int v = c.slot; v < P.n; v += c.nslots) r1[GI(v)] = 0.0;
+        for (int v = c.slot; v < P.n; v += c.nslots) glb(ar.r1)[GI(v)] = 0.0;
         __syncthreads();
-        kkt_solve<SN>(P, c, D, Av, Gv, wm, socw, soceta, r1, bb, hh, x, dy, dz, tm, gm, e1, e2, rhs, Ls, invD, O.nref);
-        for (int r = c.slot; r < P.m; r += c.nslots) s[GI(r)] = -dz[GI(r)];
+        kkt_solve<SN>(P, c, glb(ar.bb), glb(ar.hh), glb(ar.x), glb(ar.dy), glb(ar.dz), O.nref);
+        for (int r = c.slot; r < P.m; r += c.nslots) glb(ar.s)[GI(r)] = -glb(ar.dz)[GI(r)];
         __syncthreads();
         {
-            double vv[1] = {cone_shift_partial(P, c, s)};
+            double vv[1] = {cone_shift_partial(P, c, glb(ar.s))};
             double w2[1] = {0.0};
-            for (int r = c.slot; r < P.m; r += c.nslots) w2[0] += s[GI(r)] * s[GI(r)];
+            for (int r = c.slot; r < P.m; r += c.nslots) w2[0] += glb(ar.s)[GI(r)] * glb(ar.s)[GI(r)];
             seed_reduce<1>(c, vv, 2);
             const double ts = s_out[sg];
             __syncthreads();
@@ -1330,21 +1493,21 @@ restart_cold:
             const double ns = sqrt(s_out[sg]);
             if (ts >= -1e-8 * fmax(1.0, ns)) {
                 const double sh = 1.0 + ts;
-                for (int r = c.slot; r < P.l; r += c.nslots) s[GI(r)] += sh;
-                for (int k = c.slot; k < P.nsoc; k += c.nslots) s[GI(P.soc_off[k])] += sh;
+                for (int r = c.slot; r < P.l; r += c.nslots) glb(ar.s)[GI(r)] += sh;
+                for (int k = c.slot; k < P.nsoc; k += c.nslots) glb(ar.s)[GI(P.soc_off[k])] += sh;
             }
             __syncthreads();
         }
         // solve 2: [-c;0;0] -> y, z
-        for (int v = c.slot; v < P.n; v += c.nslots) r1[GI(v)] = -cc[GI(v)];
-        for (int r = c.slot; r < P.p; r += c.nslots) r2[GI(r)] = 0.0;
-        for (int r = c.slot; r < P.m; r += c.nslots) rz[GI(r)] = 0.0;
+        for (int v = c.slot; v < P.n; v += c.nslots) glb(ar.r1)[GI(v)] = -glb(ar.cc)[GI(v)];
+        for (int r = c.slot; r < P.p; r += c.nslots) glb(ar.r2)[GI(r)] = 0.0;
+        for (int r = c.slot; r < P.m; r += c.nslots) glb(ar.rz)[GI(r)] = 0.0;
         __syncthreads();
-        kkt_solve<SN>(P, c, D, Av, Gv, wm, socw, soceta, r1, r2, rz, dx, y, z, tm, gm, e1, e2, rhs, Ls, invD, O.nref);
+        kkt_solve<SN>(P, c, glb(ar.r2), glb(ar.rz), glb(ar.dx), glb(ar.y), glb(ar.z), O.nref);
         {
-            double vv[1] = {cone_shift_partial(P, c, z)};
+            double vv[1] = {cone_shift_partial(P, c, glb(ar.z))};
             double w2[1] = {0.0};
-            for (int r = c.slot; r < P.m; r += c.nslots) w2[0] += z[GI(r)] * z[GI(r)];
+            for (int r = c.slot; r < P.m; r += c.nslots) w2[0] += glb(ar.z)[GI(r)] * glb(ar.z)[GI(r)];
             seed_reduce<1>(c, vv, 2);
             const double tz = s_out[sg];
             __syncthreads();
@@ -1352,8 +1515,8 @@ restart_cold:
             const double nz = sqrt(s_out[sg]);
             if (tz >= -1e-8 * fmax(1.0, nz)) {
                 const double sh = 1.0 + tz;
-                for (int r = c.slot; r < P.l; r += c.nslots) z[GI(r)] += sh;
-                for (int k = c.slot; k < P.nsoc; k += c.nslots) z[GI(P.soc_off[k])] += sh;
+                for (int r = c.slot; r < P.l; r += c.nslots) glb(ar.z)[GI(r)] += sh;
+                for (int k = c.slot; k < P.nsoc; k += c.nslots) glb(ar.z)[GI(P.soc_off[k])] += sh;
             }
             __syncthreads();
         }
@@ -1362,12 +1525,12 @@ restart_cold:
     }
     if (s_warm[sg]) {
         const bool eq = O.equil > 0;
-        for (int i = c.slot; i < P.n; i += c.nslots) x[GI(i)] = eq ? D.xw[g * (size_t)P.n * G + GI(i)] / eqD[GI(i)] : D.xw[g * (size_t)P.n * G + GI(i)];
-        for (int i = c.slot; i < P.p; i += c.nslots) y[GI(i)] = eq ? D.yw[g * (size_t)P.p * G + GI(i)] / eqA[GI(i)] : D.yw[g * (size_t)P.p * G + GI(i)];
+        for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.x)[GI(i)] = eq ? D.xw[g * (size_t)P.n * G + GI(i)] / glb(ar.eqD)[GI(i)] : D.xw[g * (size_t)P.n * G + GI(i)];
+        for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.y)[GI(i)] = eq ? D.yw[g * (size_t)P.p * G + GI(i)] / glb(ar.eqA)[GI(i)] : D.yw[g * (size_t)P.p * G + GI(i)];
         for (int i = c.slot; i < P.m; i += c.nslots) {
-            const double e_ = eq ? eqG[GI(i)] : 1.0;
-            z[GI(i)] = D.zw[g * (size_t)P.m * G + GI(i)] / e_;
-            s[GI(i)] = D.sw[g * (size_t)P.m * G + GI(i)] * e_;
+            const double e_ = eq ? glb(ar.eqG)[GI(i)] : 1.0;
+            glb(ar.z)[GI(i)] = D.zw[g * (size_t)P.m * G + GI(i)] / e_;
+            glb(ar.s)[GI(i)] = D.sw[g * (size_t)P.m * G + GI(i)] * e_;
         }
     }
     __syncthreads();
@@ -1377,31 +1540,26 @@ restart_cold:
         // ---- residuals + objective pieces ----
         // v[7..9]: |A'y + G'z|^2, |Ax|^2, |Gx + s|^2 for the infeasibility certificates (ECOS reports INFEASIBLE /
         // DUAL_INFEASIBLE the same way; src/solvers/scp.jl:470-473 and :975 branch on those statuses)
+        // (rx, ry, rz are written by the thread that reads them back here: no barrier in between)
+        spmv_residuals();
         double v[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
         for (int i = c.slot; i < P.n; i += c.nslots) {
-            const double ci_ = cc[GI(i)];
-            const double r = ci_ + col_dot(P.At_rp, P.At_ri, P.At_vi, Av, y, i, G, sg) +
-                             col_dot(P.Gt_rp, P.Gt_ri, P.Gt_vi, Gv, z, i, G, sg);
-            rx[GI(i)] = r;
+            const double ci_ = glb(ar.cc)[GI(i)], r = glb(ar.rx)[GI(i)];
             v[0] += r * r;
-            v[3] += ci_ * x[GI(i)];
+            v[3] += ci_ * glb(ar.x)[GI(i)];
             v[7] += (r - ci_) * (r - ci_);
         }
         for (int i = c.slot; i < P.p; i += c.nslots) {
-            const double bi_ = bb[GI(i)];
-            const double r = row_dot(P.A_rp, P.A_ci, Av, x, i, G, sg) - bi_;
-            ry[GI(i)] = r;
+            const double bi_ = glb(ar.bb)[GI(i)], r = glb(ar.ry)[GI(i)];
             v[1] += r * r;
-            v[4] += bi_ * y[GI(i)];
+            v[4] += bi_ * glb(ar.y)[GI(i)];
             v[8] += (r + bi_) * (r + bi_);
         }
         for (int i = c.slot; i < P.m; i += c.nslots) {
-            const double hi_ = hh[GI(i)];
-            const double r = row_dot(P.G_rp, P.G_ci, Gv, x, i, G, sg) + s[GI(i)] - hi_;
-            rz[GI(i)] = r;
+            const double hi_ = glb(ar.hh)[GI(i)], r = glb(ar.rz)[GI(i)];
             v[2] += r * r;
-            v[5] += hi_ * z[GI(i)];
-            v[6] += s[GI(i)] * z[GI(i)];
+            v[5] += hi_ * glb(ar.z)[GI(i)];
+            v[6] += glb(ar.s)[GI(i)] * glb(ar.z)[GI(i)];
             v[9] += (r + hi_) * (r + hi_);
         }
         seed_reduce<10>(c, v, 0);
@@ -1454,18 +1612,18 @@ restart_cold:
         }
         __syncthreads();
         if (s_save[sg]) {
-            for (int i = c.slot; i < P.n; i += c.nslots) xb[GI(i)] = x[GI(i)];
-            for (int i = c.slot; i < P.p; i += c.nslots) yb[GI(i)] = y[GI(i)];
-            for (int i = c.slot; i < P.m; i += c.nslots) { zb[GI(i)] = z[GI(i)]; sb[GI(i)] = s[GI(i)]; }
+            for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.xb)[GI(i)] = glb(ar.x)[GI(i)];
+            for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.yb)[GI(i)] = glb(ar.y)[GI(i)];
+            for (int i = c.slot; i < P.m; i += c.nslots) { glb(ar.zb)[GI(i)] = glb(ar.z)[GI(i)]; glb(ar.sb)[GI(i)] = glb(ar.s)[GI(i)]; }
         }
         if (s_wsave[sg]) {   // in the caller's units (the next program is equilibrated differently)
             const bool eq = O.equil > 0;
-            for (int i = c.slot; i < P.n; i += c.nslots) D.xw[g * (size_t)P.n * G + GI(i)] = eq ? x[GI(i)] * eqD[GI(i)] : x[GI(i)];
-            for (int i = c.slot; i < P.p; i += c.nslots) D.yw[g * (size_t)P.p * G + GI(i)] = eq ? y[GI(i)] * eqA[GI(i)] : y[GI(i)];
+            for (int i = c.slot; i < P.n; i += c.nslots) D.xw[g * (size_t)P.n * G + GI(i)] = eq ? glb(ar.x)[GI(i)] * glb(ar.eqD)[GI(i)] : glb(ar.x)[GI(i)];
+            for (int i = c.slot; i < P.p; i += c.nslots) D.yw[g * (size_t)P.p * G + GI(i)] = eq ? glb(ar.y)[GI(i)] * glb(ar.eqA)[GI(i)] : glb(ar.y)[GI(i)];
             for (int i = c.slot; i < P.m; i += c.nslots) {
-                const double e_ = eq ? eqG[GI(i)] : 1.0;
-                D.zw[g * (size_t)P.m * G + GI(i)] = z[GI(i)] * e_;
-                D.sw[g * (size_t)P.m * G + GI(i)] = s[GI(i)] / e_;
+                const double e_ = eq ? glb(ar.eqG)[GI(i)] : 1.0;
+                D.zw[g * (size_t)P.m * G + GI(i)] = glb(ar.z)[GI(i)] * e_;
+                D.sw[g * (size_t)P.m * G + GI(i)] = glb(ar.s)[GI(i)] / e_;
             }
         }
         __syncthreads();
@@ -1479,7 +1637,7 @@ restart_cold:
         PROF(2)
 
         // ---- scaling, KKT assembly, factorisation ----
-        nt_scaling(P, c, s, z, lam, wm, socw, soceta);
+        nt_scaling(P, c, glb(ar.s), glb(ar.z), glb(ar.lam), glb(ar.wm), glb(ar.socw), glb(ar.soceta));
         __syncthreads();
         PROF(3)
         IPM_FACTOR()
@@ -1487,24 +1645,24 @@ restart_cold:
         if (c.tid == 0) ipm_s_prof[11]++;
 
         // ---- affine direction: bx=-rx, by=-ry, bz=-rz+s ; ds = -s - W^2 dz ----
-        for (int i = c.slot; i < P.n; i += c.nslots) r1[GI(i)] = -rx[GI(i)];
-        for (int i = c.slot; i < P.p; i += c.nslots) r2[GI(i)] = -ry[GI(i)];
-        for (int i = c.slot; i < P.m; i += c.nslots) ds[GI(i)] = -rz[GI(i)] + s[GI(i)];  // ds used as bz scratch
+        for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.r1)[GI(i)] = -glb(ar.rx)[GI(i)];
+        for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.r2)[GI(i)] = -glb(ar.ry)[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) glb(ar.ds)[GI(i)] = -glb(ar.rz)[GI(i)] + glb(ar.s)[GI(i)];  // ds used as bz scratch
         __syncthreads();
         PROF(6)
-        kkt_solve<SN>(P, c, D, Av, Gv, wm, socw, soceta, r1, r2, ds, dx, dy, dza, tm, gm, e1, e2, rhs, Ls, invD, O.nref_aff);
+        kkt_solve<SN>(P, c, glb(ar.r2), glb(ar.ds), glb(ar.dx), glb(ar.dy), glb(ar.dza), O.nref_aff);
         PROF(5)
         // ds = tmp - W^2 dz with tmp = -s; W^2 dz == G dx - bz is left in gm by kkt_solve (no W^2 W^-2
         // round trip: keeps G dx + ds = -rz to rounding even when the scaling is ill-conditioned)
-        for (int i = c.slot; i < P.m; i += c.nslots) dsa[GI(i)] = -s[GI(i)] - gm[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) glb(ar.dsa)[GI(i)] = -glb(ar.s)[GI(i)] - glb(ar.gm)[GI(i)];
         __syncthreads();
         {   // separate primal / dual step lengths (the primal and dual residuals shrink independently); centring
             // parameter from the predicted complementarity, sigma = (mu_aff / mu)^3 (Mehrotra)
-            double a[2] = {cone_alpha_partial(P, c, s, dsa), cone_alpha_partial(P, c, z, dza)};
+            double a[2] = {cone_alpha_partial(P, c, glb(ar.s), glb(ar.dsa)), cone_alpha_partial(P, c, glb(ar.z), glb(ar.dza))};
             seed_reduce<2>(c, a, 1);
             const double ap = fmin(1.0, s_out[sg]), ad = fmin(1.0, s_out[IPM_MAXG + sg]);
             double ma[1] = {0.0};
-            for (int i = c.slot; i < P.m; i += c.nslots) ma[0] = fma(s[GI(i)] + ap * dsa[GI(i)], z[GI(i)] + ad * dza[GI(i)], ma[0]);
+            for (int i = c.slot; i < P.m; i += c.nslots) ma[0] = fma(glb(ar.s)[GI(i)] + ap * glb(ar.dsa)[GI(i)], glb(ar.z)[GI(i)] + ad * glb(ar.dza)[GI(i)], ma[0]);
             seed_reduce<1>(c, ma, 0);
             if (c.tid < G) {
                 double r = s_out[c.tid] / (deg * s_mu[c.tid]);
@@ -1517,26 +1675,26 @@ restart_cold:
             __syncthreads();
         }
         // ---- combined direction ----
-        combined_tmp(P, c, s, z, lam, socw, soceta, dsa, dza, s_sigmu, tm);
+        combined_tmp(P, c, glb(ar.s), glb(ar.z), glb(ar.lam), glb(ar.socw), glb(ar.soceta), glb(ar.dsa), glb(ar.dza), s_sigmu, glb(ar.tm));
         __syncthreads();
         {
             const double sc = s_scale[sg];
-            for (int i = c.slot; i < P.n; i += c.nslots) r1[GI(i)] = -sc * rx[GI(i)];
-            for (int i = c.slot; i < P.p; i += c.nslots) r2[GI(i)] = -sc * ry[GI(i)];
+            for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.r1)[GI(i)] = -sc * glb(ar.rx)[GI(i)];
+            for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.r2)[GI(i)] = -sc * glb(ar.ry)[GI(i)];
             for (int i = c.slot; i < P.m; i += c.nslots) {
-                const double t = tm[GI(i)];
-                dsa[GI(i)] = t;                        // keep tmp
-                ds[GI(i)] = -sc * rz[GI(i)] - t;       // bz
+                const double t = glb(ar.tm)[GI(i)];
+                glb(ar.dsa)[GI(i)] = t;                        // keep tmp
+                glb(ar.ds)[GI(i)] = -sc * glb(ar.rz)[GI(i)] - t;       // bz
             }
         }
         __syncthreads();
         PROF(6)
-        kkt_solve<SN>(P, c, D, Av, Gv, wm, socw, soceta, r1, r2, ds, dx, dy, dz, tm, gm, e1, e2, rhs, Ls, invD, O.nref);
+        kkt_solve<SN>(P, c, glb(ar.r2), glb(ar.ds), glb(ar.dx), glb(ar.dy), glb(ar.dz), O.nref);
         PROF(5)
-        for (int i = c.slot; i < P.m; i += c.nslots) ds[GI(i)] = dsa[GI(i)] - gm[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) glb(ar.ds)[GI(i)] = glb(ar.dsa)[GI(i)] - glb(ar.gm)[GI(i)];
         __syncthreads();
         {
-            double a[2] = {cone_alpha_partial(P, c, s, ds), cone_alpha_partial(P, c, z, dz)};
+            double a[2] = {cone_alpha_partial(P, c, glb(ar.s), glb(ar.ds)), cone_alpha_partial(P, c, glb(ar.z), glb(ar.dz))};
             seed_reduce<2>(c, a, 1);
             if (c.tid < G) {
                 s_alpha[c.tid] = s_done[c.tid] ? 0.0 : fmin(1.0, 0.99 * s_out[c.tid]);                 // primal: x, s
@@ -1547,7 +1705,7 @@ restart_cold:
         // safeguard: make sure the new point is strictly interior (halve the step otherwise) so that the
         // next NT scaling is well defined
         for (int bt = 0; bt < 12; bt++) {
-            double mg[2] = {cone_margin_partial(P, c, s, ds, s_alpha[sg]), cone_margin_partial(P, c, z, dz, s_alpha_d[sg])};
+            double mg[2] = {cone_margin_partial(P, c, glb(ar.s), glb(ar.ds), s_alpha[sg]), cone_margin_partial(P, c, glb(ar.z), glb(ar.dz), s_alpha_d[sg])};
             seed_reduce<2>(c, mg, 1);
             if (c.tid == 0) s_alldone = 1;
             __syncthreads();
@@ -1563,12 +1721,12 @@ restart_cold:
         {
             const double ap = s_alpha[sg], ad = s_alpha_d[sg];
             if (ap > 0.0) {
-                for (int i = c.slot; i < P.n; i += c.nslots) x[GI(i)] += ap * dx[GI(i)];
-                for (int i = c.slot; i < P.m; i += c.nslots) s[GI(i)] += ap * ds[GI(i)];
+                for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.x)[GI(i)] += ap * glb(ar.dx)[GI(i)];
+                for (int i = c.slot; i < P.m; i += c.nslots) glb(ar.s)[GI(i)] += ap * glb(ar.ds)[GI(i)];
             }
             if (ad > 0.0) {
-                for (int i = c.slot; i < P.p; i += c.nslots) y[GI(i)] += ad * dy[GI(i)];
-                for (int i = c.slot; i < P.m; i += c.nslots) z[GI(i)] += ad * dz[GI(i)];
+                for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.y)[GI(i)] += ad * glb(ar.dy)[GI(i)];
+                for (int i = c.slot; i < P.m; i += c.nslots) glb(ar.z)[GI(i)] += ad * glb(ar.dz)[GI(i)];
             }
         }
         __syncthreads();
@@ -1611,15 +1769,15 @@ restart_cold:
     }
     __syncthreads();
     if (s_best[sg] < CUDART_INF) {
-        for (int i = c.slot; i < P.n; i += c.nslots) x[GI(i)] = xb[GI(i)];
-        for (int i = c.slot; i < P.p; i += c.nslots) y[GI(i)] = yb[GI(i)];
-        for (int i = c.slot; i < P.m; i += c.nslots) { z[GI(i)] = zb[GI(i)]; s[GI(i)] = sb[GI(i)]; }
+        for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.x)[GI(i)] = glb(ar.xb)[GI(i)];
+        for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.y)[GI(i)] = glb(ar.yb)[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) { glb(ar.z)[GI(i)] = glb(ar.zb)[GI(i)]; glb(ar.s)[GI(i)] = glb(ar.sb)[GI(i)]; }
     }
     if (O.equil > 0) {  // back to the caller's units
         __syncthreads();
-        for (int i = c.slot; i < P.n; i += c.nslots) x[GI(i)] *= eqD[GI(i)];
-        for (int i = c.slot; i < P.p; i += c.nslots) y[GI(i)] *= eqA[GI(i)];
-        for (int i = c.slot; i < P.m; i += c.nslots) { z[GI(i)] *= eqG[GI(i)]; s[GI(i)] /= eqG[GI(i)]; }
+        for (int i = c.slot; i < P.n; i += c.nslots) glb(ar.x)[GI(i)] *= glb(ar.eqD)[GI(i)];
+        for (int i = c.slot; i < P.p; i += c.nslots) glb(ar.y)[GI(i)] *= glb(ar.eqA)[GI(i)];
+        for (int i = c.slot; i < P.m; i += c.nslots) { glb(ar.z)[GI(i)] *= glb(ar.eqG)[GI(i)]; glb(ar.s)[GI(i)] /= glb(ar.eqG)[GI(i)]; }
     }
     if (c.tid < G) {
         const int sd = (int)g * G + c.tid;
